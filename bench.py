@@ -1,5 +1,5 @@
 #!/usr/bin/env python
-"""bench.py -- resquiggle throughput of the B200-native hot path.
+"""bench.py -- resquiggle throughput of the CUDA hot path on one or more H100s.
 
     python bench.py --gpus N --steps K --warmup W            (ours; torchrun for N > 1)
     python bench.py --impl reference --gpus N --steps K --warmup W
@@ -23,6 +23,11 @@ BASELINE.json shapes (configs[2] mixed 2k-20k / bw 400 + rescue, configs[3] dire
 
     python bench.py --workload mixed --queue --reads R       strong scaling over a shared
                                                              NCCL-free queue of length buckets
+
+--dump-outputs DIR writes the headline workload's results of the last timed end-to-end step
+as DIR/<name>.npy (float64): every per-read field of a fixed, seeded sample of up to 150k
+reads and the segments / per-base means of a smaller seeded sample (at most 64 MB in all),
+so that two builds can be compared output for output on identical inputs.
 """
 import argparse
 import json
@@ -57,7 +62,7 @@ CONFIGS = {
                label='configs[1]: %d synthetic DNA reads/GPU x ~4k samples (444 bases, 6-mer '
                      'model), bandwidth=200, default start params => static-band path W~748, '
                      'float64 raw'),
-    'mixed': dict(kind='DNA', aln=ALN_MIXED, seg=SEG_DNA, nbases='mixed', reads=40000, parity=512,
+    'mixed': dict(kind='DNA', aln=ALN_MIXED, seg=SEG_DNA, nbases='mixed', reads=20000, parity=512,
                   cpu_single=8, cpu_pool_per_core=4,
                   label='configs[2]-like: %d synthetic DNA reads/GPU, 2k-20k samples (222-2222 '
                         'bases), bandwidth=400 adaptive band + save-bandwidth rescue, float64 raw'),
@@ -139,7 +144,7 @@ def peaks():
             return float(json.load(open(p))['hbm_gbs']), 'measured (MEASURED_PEAKS.json)'
         except Exception:
             pass
-    return 6650.0, 'fallback (B200_PROFILING.md)'
+    return 3350.0, 'H100 SXM data sheet (HBM3, 3.35 TB/s)'
 
 
 class ClockSampler(object):
@@ -487,28 +492,30 @@ def reduce_sum(dist, x):
     return float(t[0])
 
 
-def traffic_per_read():
-    """measured DRAM bytes per read of the dominant kernel from this round's ncu capture
-    (profiles/k_align_traffic.json); None when the capture predates the current kernel source
-    (the file stores a hash of csrc/dp_*.cuh), so a stale constant never reaches the line"""
-    import hashlib
-    tp = os.path.join(REPO, 'profiles', 'k_align_traffic.json')
-    try:
-        t = json.load(open(tp))
-    except Exception:
-        return None, 'no capture'
-    h = hashlib.sha256()
-    for f in ('dp_row.cuh', 'dp_align.cuh', 'dp_align_kernel.cuh', 'dp_row2.cuh', 'common.cuh'):
-        p = os.path.join(REPO, 'tombo_b200', 'csrc', f)
-        if os.path.exists(p):
-            h.update(open(p, 'rb').read())
-    if t.get('source_sha16') != h.hexdigest()[:16]:
-        return None, 'capture predates the current kernel source'
-    return t.get('dram_bytes_per_read'), t.get('capture', 'ncu --set full')
+def dump_outputs(d, out, seq_off, k, n_reads):
+    """write the results in `out` as d/<name>.npy, float64: per-read fields of a seeded sample
+    of <= 150k reads (<= 14 MB), segs / norm_mean of a seeded sample of <= 6M values (48 MB)"""
+    os.makedirs(d, exist_ok=True)
+    nb = (seq_off[1:] - seq_off[:-1]) - (k - 1)
+    rs = np.random.RandomState(20240)
+    per_read = np.sort(rs.choice(n_reads, min(n_reads, 150000), replace=False))
+    np.save(os.path.join(d, 'read_index.npy'), per_read.astype(np.float64))
+    for f in ('status', 'n_iters', 'flags', 'read_start_rel_to_raw', 'sig_match_score',
+              'scale_values'):
+        np.save(os.path.join(d, f + '.npy'), out[f][per_read].astype(np.float64))
+    m = int(min(n_reads, max(1, 6000000 // (2 * int(nb.max()) + 1))))
+    sub = np.sort(rs.choice(n_reads, m, replace=False))
+    seg_off = np.concatenate([[0], np.cumsum(nb + 1)])
+    base_off = np.concatenate([[0], np.cumsum(nb)])
+    np.save(os.path.join(d, 'segs_read_index.npy'), sub.astype(np.float64))
+    np.save(os.path.join(d, 'segs.npy'), np.concatenate(
+        [out['segs'][seg_off[i]:seg_off[i + 1]] for i in sub]).astype(np.float64))
+    np.save(os.path.join(d, 'norm_mean.npy'), np.concatenate(
+        [out['norm_mean'][base_off[i]:base_off[i + 1]] for i in sub]).astype(np.float64))
 
 
 def run_config(name, n_reads, steps, warmup, ctx, rank, local, dist, n_gpus, pin, do_parity=True,
-               int16_e2e=False):
+               int16_e2e=False, dump_dir=None):
     """warm-up, timed resident region (device clock), timed end-to-end region (host buffers),
     parity sample -- for one workload.  Returns the fields of the JSON line."""
     from tombo_b200 import _lib, synthetic as syn
@@ -594,6 +601,8 @@ def run_config(name, n_reads, steps, warmup, ctx, rank, local, dist, n_gpus, pin
         reg = e2e_step(raw)
     t_e2e = time.perf_counter() - t0
     barrier(dist)
+    if dump_dir and rank == 0:
+        dump_outputs(dump_dir, out, seq_off, k, n_reads)
     t_dev = reduce_max(dist, dev_ms / 1e3)
     t_res_w = reduce_max(dist, t_res)
     t_e2e_w = reduce_max(dist, t_e2e)
@@ -624,8 +633,6 @@ def run_config(name, n_reads, steps, warmup, ctx, rank, local, dist, n_gpus, pin
     peak, peak_src = peaks()
     bytes_per_read = float(a_dp.mean())
     ach = bytes_per_read * dp_reads / (dp_ms / 1e3) / 1e9 if dp_ms > 0 else 0.0
-    tpr, tsrc = traffic_per_read()
-    traffic = tpr * dp_reads / max(1.0, dp_launches) if (tpr and name == 'c1') else None
     res = {
         'metric': METRIC, 'value': tot_reads / t_dev, 'unit': 'reads/s',
         'samples_per_sec': tot_samples / t_dev,
@@ -634,15 +641,14 @@ def run_config(name, n_reads, steps, warmup, ctx, rank, local, dist, n_gpus, pin
         'scaling': 'weak', 'vs_baseline': None, 'dtype': 'f64', 'data': 'synthetic',
         'config': {'workload': cfg['label'] % n_reads, 'reads_per_gpu': n_reads,
                    'parallelism': 'reads sharded over %d GPU(s), no collective' % n_gpus,
-                   'l2': 'inputs %.2f GB per step >> 126 MB L2 (no flush needed)'
+                   'l2': 'inputs %.2f GB per step >> 50 MB L2 (no flush needed)'
                          % (raw.nbytes / 1e9),
                    'value_wall_clock_reads_per_s': tot_reads / t_res_w,
                    'reads_ok_frac': tot_ok / (tot_reads / steps),
                    'reads_rescued': n_rescued},
         'roofline': {'bound': 'hbm', 'kernel': 'k_align (banded DP + traceback)',
                      'achieved': ach, 'peak': peak, 'unit': 'GB/s',
-                     'frac': ach / peak, 'traffic': traffic, 'traffic_source': tsrc,
-                     'peak_source': peak_src,
+                     'frac': ach / peak, 'peak_source': peak_src,
                      'algorithmic_bytes_per_read': bytes_per_read,
                      'launches': dp_launches, 'avg_launch_ms': dp_ms / max(1.0, dp_launches),
                      'dp_share_of_step': dp_ms / max(1e-9, dev_ms),
@@ -842,6 +848,8 @@ def main():
     ap.add_argument('--queue-threads', type=int, default=4,
                     help='worker threads (one library context each) per rank in --queue mode')
     ap.add_argument('--bucket-samples', type=int, default=60_000_000)
+    ap.add_argument('--dump-outputs', default='', metavar='DIR',
+                    help='write the headline results of the last timed step as DIR/<name>.npy')
     ap.add_argument('--cpu-leg', default='', help=argparse.SUPPRESS)
     ap.add_argument('--cpu-scale', type=float, default=1.0, help=argparse.SUPPRESS)
     args = ap.parse_args()
@@ -909,7 +917,8 @@ def main():
         while pinned:
             pinned.pop().free()
     line = run_config(args.workload, n_reads, args.steps, args.warmup, ctx, rank, local, dist,
-                      args.gpus, pin, do_parity=not args.no_parity, int16_e2e=not args.no_int16)
+                      args.gpus, pin, do_parity=not args.no_parity, int16_e2e=not args.no_int16,
+                      dump_dir=args.dump_outputs)
     free_pinned()
     if rank == 0:
         line['config']['numa'] = numa
@@ -920,6 +929,10 @@ def main():
             line['cpu_baseline'] = cpu_baseline_obj(leg, args.workload)
     ex_out = []
     for e in extras:
+        # a fresh context per workload: device pools are grow-only, so the previous workload's
+        # buffers would otherwise stay allocated beside this one's on an 80 GB device
+        ctx.close()
+        ctx = _lib.Context(local)
         try:
             r = run_config(e, CONFIGS[e]['reads'], args.extra_steps, max(3, min(args.warmup, 3)),
                            ctx, rank, local, dist, args.gpus, pin, do_parity=not args.no_parity)

@@ -1,11 +1,11 @@
-/* tombo_b200.h -- C ABI of the B200-native resquiggle engine.
+/* tombo_b200.h -- C ABI of the CUDA resquiggle engine (NVIDIA H100, sm_90a).
  *
  * Drop-in boundary for the native layer of nanoporetech/tombo's resquiggle hot
  * path: it replaces the two Cython extension modules
  *   tombo/_c_dynamic_programming.pyx   and   tombo/_c_helper.pyx
  * (built by the reference's setup.py:51-62) plus the per-read numpy glue of
  * tombo/resquiggle.py:345-1214 and tombo/tombo_stats.py:203-573, 2327-2370,
- * 3972-4082 with hand-written CUDA for sm_100a.
+ * 3972-4082 with hand-written CUDA for sm_90a.
  *
  * Conventions
  *   - plain C: pointers + sizes, no torch / numpy types.
@@ -20,7 +20,7 @@
  *     1..21 map 1:1 onto the reference's TomboError / NotImplementedError message
  *     strings (tb2_status_message); the reference raises, we return.
  *   - there is NO CPU fallback: every entry point runs CUDA kernels and fails with
- *     TB2_ERR_CUDA if no sm_100-class device is usable.
+ *     TB2_ERR_CUDA if no sm_90-class device is usable.
  */
 #ifndef TOMBO_B200_H
 #define TOMBO_B200_H

@@ -11,7 +11,7 @@ for p in (REPO, os.path.join(REPO, 'oracle')):
 
 
 def pytest_configure(config):
-    config.addinivalue_line('markers', 'gpu: needs a CUDA device (B200)')
+    config.addinivalue_line('markers', 'gpu: needs a CUDA device (H100)')
 
 
 @pytest.fixture(scope='session')

@@ -3,7 +3,7 @@
 // user-level fiber (ucontext), warp collectives (__shfl*_sync, __any_sync,
 // __ballot_sync, __syncwarp) and __syncthreads are rendezvous points between the
 // fibers.  It lets the CPU test-suite run the *same device source* (csrc/*.cuh) that
-// nvcc compiles for sm_100a and compare it with the oracle -- an algorithm check for
+// nvcc compiles for sm_90a and compare it with the oracle -- an algorithm check for
 // index / band / edge-case logic before GPU time is spent.  Never linked into
 // libtombo_b200.so; the product path has no CPU fallback.
 #pragma once

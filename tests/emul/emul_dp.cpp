@@ -1,6 +1,6 @@
 // emul_dp.cpp -- TEST INFRASTRUCTURE ONLY: runs the device source of the banded-DP
 // assignment kernel (tombo_b200/csrc/dp_align_kernel.cuh, the file nvcc compiles for
-// sm_100a) on the host through tests/emul/cuda_emul.h, so the CPU test-suite can compare
+// sm_90a) on the host through tests/emul/cuda_emul.h, so the CPU test-suite can compare
 // the kernel's logic with the oracle.  Not part of libtombo_b200.so.
 #include "cuda_emul.h"
 #include "../../tombo_b200/csrc/dp_align_kernel.cuh"

@@ -1,4 +1,6 @@
 """Helpers to replay tests/golden/*.npz (outputs of the unmodified reference)."""
+import gzip
+import json
 import os
 
 import numpy as np
@@ -16,6 +18,11 @@ DNA_SEG, RNA_SEG = (5, 3, 1, 5), (12, 6, 2, 15)
 
 def load(name):
     return np.load(os.path.join(GOLDEN, name + '.npz'), allow_pickle=False)
+
+
+def load_json(name):
+    with gzip.open(os.path.join(GOLDEN, name + '.json.gz'), 'rt') as f:
+        return json.load(f)
 
 
 def reads_of(g):

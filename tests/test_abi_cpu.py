@@ -60,29 +60,27 @@ def test_python_api_surface_imports_without_gpu():
     assert m.motif_pat.pattern == 'CC[AT]GG' and m.mod_base == 'C'
 
 
+NAMEDTUPLES = ('alignInfo', 'readData', 'scaleValues', 'resquiggleParams', 'resquiggleResults',
+               'dpResults', 'genomeLocation', 'seqSampleType', 'stallParams', 'channelInfo')
+
+
 def test_parameters_and_namedtuples_match_reference_when_available():
-    import sys, os
-    sys.path.insert(0, os.path.join(REPO, 'oracle'))
-    import ref_harness as rh
-    if not rh.available():
-        pytest.skip('oracle/_ref not built')
-    m = rh.load_reference()
+    """against the reference's values stored by tests/golden/make_shim_golden.py"""
+    import json
+    import golden_util as gu
     from tombo_b200 import tombo_helper as th, tombo_stats as ts, _default_parameters as dp
-    import tombo._default_parameters as rdp
+    ref = gu.load_json('shim_reference')
     for name in dir(dp):
         if name.isupper():
-            assert getattr(dp, name) == getattr(rdp, name), name
-    for nt in ('alignInfo', 'readData', 'scaleValues', 'resquiggleParams', 'resquiggleResults',
-               'dpResults', 'genomeLocation', 'seqSampleType', 'stallParams', 'channelInfo'):
-        assert getattr(th, nt)._fields == getattr(m['th'], nt)._fields, nt
+            assert json.loads(json.dumps(getattr(dp, name))) == ref['default_parameters'][name], name
+    for nt in NAMEDTUPLES:
+        assert list(getattr(th, nt)._fields) == ref['namedtuple_fields'][nt], nt
     for kind in ('DNA', 'RNA'):
         sst = th.seqSampleType(kind, kind == 'RNA')
         for save in (False, True):
             a = ts.load_resquiggle_parameters(sst, use_save_bandwidth=save)
-            b = m['ts'].load_resquiggle_parameters(m['th'].seqSampleType(kind, kind == 'RNA'),
-                                                   use_save_bandwidth=save)
-            assert tuple(a) == tuple(b)
-    assert ts.HALF_NORM_EXPECTED_VAL == m['ts'].HALF_NORM_EXPECTED_VAL
+            assert tuple(a) == tuple(ref['resquiggle_parameters']['%s_%d' % (kind, save)])
+    assert ts.HALF_NORM_EXPECTED_VAL == ref['HALF_NORM_EXPECTED_VAL']
 
 
 def test_pipeline_chunk_schedule_covers_every_read_once():
@@ -94,7 +92,7 @@ def test_pipeline_chunk_schedule_covers_every_read_once():
     fn.restype = ctypes.c_int
     fn.argtypes = [ctypes.c_int, ctypes.c_int64, ctypes.POINTER(ctypes.c_int64), ctypes.c_int]
     buf = (ctypes.c_int64 * 4096)()
-    sm = 148
+    sm = 132                              # H100 SXM
     unit = sm * 32
     for n in [0, 1, unit, 6 * unit, 6 * unit + 1, 39122, 100000, 1000003]:
         k = fn(sm, n, buf, 4096)

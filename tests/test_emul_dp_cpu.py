@@ -1,5 +1,5 @@
 """CPU: the banded-DP device source (tombo_b200/csrc/dp_*.cuh, the files nvcc compiles for
-sm_100a) executed on the host emulation of tests/emul and compared bit for bit with the
+sm_90a) executed on the host emulation of tests/emul and compared bit for bit with the
 oracle's find_adaptive_base_assignment -- static band, start search, masked start,
 adaptive rows, traceback.  An algorithm check of the kernel source; the GPU parity tests
 remain the proof for the compiled kernel."""

@@ -139,7 +139,7 @@ def test_large_batch_pipelined_chunks_match_single_chunk(ctx, dna_model, RPcls):
     kmer_ref, cpos = dna_model
     means, sds = syn.kmer_table(kmer_ref)
     ctx.set_model(means, sds, 6, cpos)
-    n = 4 * 148 * 32 * 2 + 1234           # > 1.5 chunks on a 148-SM part
+    n = 4 * 132 * 32 * 2 + 1234           # > 6 x 32 reads per SM: 3 chunks on a 132-SM H100
     raw, raw_off, codes, seq_off = syn.make_read_batch(kmer_ref, n, 60, 77)
     # a few long reads so that the keyed sub-sampling (global read index) is exercised
     rp, sp = RPcls(bench.ALN_DNA), RPcls(bench.ALN_DNA, save=True)

@@ -1,8 +1,11 @@
 """CPU: host-side pieces of the Python mirror API -- batch packing (one bad read never
 aborts a batch), error typing, and the two helpers re-expressed in vectorised form checked
-against the unmodified reference (oracle/_ref) on random inputs."""
+against the unmodified reference on seeded random inputs (tests/golden/shim_reference.json.gz,
+written by tests/golden/make_shim_golden.py)."""
 import numpy as np
 import pytest
+
+import golden_util as gu
 
 
 def _map_res(raw, seq):
@@ -51,18 +54,9 @@ def test_batcher_files_library_errors_as_non_tombo():
     assert out[2][1][0] is False
 
 
-def _reference():
-    import ref_harness as rh
-    if not rh.available():
-        pytest.skip('oracle/_ref not built')
-    return rh.load_reference()
-
-
-def test_trim_seq_and_means_equals_reference_on_random_regions():
-    m = _reference()
-    from tombo_b200 import tombo_stats as ts, tombo_helper as th
+def trim_cases():
+    """seeded random regions for trim_seq_and_means: (seq, means, args)"""
     rs = np.random.RandomState(3)
-    seen = {'ok': 0, 'err': 0}
     for it in range(3000):
         K = int(rs.choice([5, 6, 7])); cp = int(rs.randint(0, K))
         L = int(rs.randint(K, 40))
@@ -72,32 +66,61 @@ def test_trim_seq_and_means_equals_reference_on_random_regions():
         reg_start = int(rs.randint(0, 60))
         args += (reg_start, reg_start + int(rs.randint(1, 60)), str(rs.choice(['+', '-'])), K, cp,
                  int(rs.randint(0, 4)), int(rs.randint(0, 8)))
-
-        def call(f, err):
-            try:
-                k, mm, r, ms = f(seq, means.copy(), *args)
-                return ('ok', list(k), mm.tolist(), r, ms)
-            except err as e:
-                return ('err', str(e))
-        a = call(m['ts'].trim_seq_and_means, m['th'].TomboError)
-        b = call(ts.trim_seq_and_means, th.TomboError)
-        assert a == b, (it, args)
-        seen[a[0]] += 1
-    assert seen['ok'] > 500 and seen['err'] > 500
+        yield seq, means, args
 
 
-def test_remove_stall_cpts_equals_reference():
-    m = _reference()
-    from tombo_b200 import resquiggle as rq
+def stall_cases():
+    """seeded random stall intervals and changepoints for remove_stall_cpts: (ints, cp)"""
     rs = np.random.RandomState(4)
     for it in range(1000):
         ns = int(rs.randint(0, 6))
         ints = np.sort(rs.choice(np.arange(0, 2000), 2 * ns, replace=False)).reshape(-1, 2)
         cp = np.sort(rs.choice(np.arange(0, 2000), int(rs.randint(1, 300)),
                                replace=False)).astype(np.int64)
-        a = m['ts'].remove_stall_cpts([tuple(x) for x in ints], cp)
-        b = rq._remove_stall_cpts([tuple(x) for x in ints], cp)
-        assert np.array_equal(a, b)
+        yield [tuple(x) for x in ints], cp
+
+
+def decode_trim(seq, means, args, g):
+    """the stored reference result: its k-mers, means and (on the + strand) sequence are
+    slices of the inputs, stored as (start, length); errors as their message"""
+    if g[0] == 'err':
+        return tuple(g)
+    _, k0, nk, m0, nm, r, ms = g
+    K = args[4]
+    if not isinstance(ms, str):
+        ms = seq[ms[0]:ms[0] + ms[1]]
+    return ('ok', [seq[k0 + j:k0 + j + K] for j in range(nk)], means[m0:m0 + nm].tolist(), r, ms)
+
+
+def test_trim_seq_and_means_equals_reference_on_random_regions():
+    from tombo_b200 import tombo_stats as ts, tombo_helper as th
+    ref = gu.load_json('shim_reference')['trim_seq_and_means']
+    seen = {'ok': 0, 'err': 0}
+    for it, (seq, means, args) in enumerate(trim_cases()):
+        try:
+            k, mm, r, ms = ts.trim_seq_and_means(seq, means.copy(), *args)
+            b = ('ok', list(k), mm.tolist(), r, ms)
+        except th.TomboError as e:
+            b = ('err', str(e))
+        a = decode_trim(seq, means, args, ref[it])
+        assert a == b, (it, args)
+        seen[a[0]] += 1
+    assert it + 1 == len(ref)
+    assert seen['ok'] > 500 and seen['err'] > 500
+
+
+def drop_runs(cp, runs):
+    """cp without the [start, end) index runs the reference dropped"""
+    return np.delete(cp, [i for a, b in runs for i in range(a, b)])
+
+
+def test_remove_stall_cpts_equals_reference():
+    from tombo_b200 import resquiggle as rq
+    ref = gu.load_json('shim_reference')['remove_stall_cpts']
+    for it, (ints, cp) in enumerate(stall_cases()):
+        b = rq._remove_stall_cpts(ints, cp)
+        assert np.array_equal(drop_runs(cp, ref[it]), b), it
+    assert it + 1 == len(ref)
 
 
 def test_write_new_fast5_group_opens_path_likes_and_always_closes(monkeypatch, tmp_path):

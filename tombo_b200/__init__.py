@@ -1,4 +1,4 @@
-"""tombo_b200 -- a B200-native (sm_100a) implementation of the Tombo resquiggle hot
+"""tombo_b200 -- a CUDA (H100, sm_90a) implementation of the Tombo resquiggle hot
 path behind the ``tombo.resquiggle`` / ``tombo.tombo_stats`` / ``tombo.tombo_helper``
 Python API.  Host code is Python calling hand-written CUDA through a C ABI
 (include/tombo_b200.h, tombo_b200/libtombo_b200.so); there is no CPU fallback.

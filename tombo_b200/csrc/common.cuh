@@ -1,4 +1,4 @@
-// common.cuh -- shared device helpers for the tombo_b200 CUDA kernels (sm_100a).
+// common.cuh -- shared device helpers for the tombo_b200 CUDA kernels (sm_90a).
 //
 // Arithmetic contract: everything that feeds an integer decision (event
 // boundaries, band placement, traceback moves) is evaluated in fp64 with the

@@ -37,7 +37,7 @@ struct DevBuf {
 
 struct tb2_ctx {
     int device = 0;
-    int sm_count = 148;
+    int sm_count = 132;            // H100 SXM; set from the device in tb2_ctx_create
     cudaStream_t stream = nullptr;
     cudaEvent_t ev0 = nullptr, ev1 = nullptr, ev2 = nullptr, ev3 = nullptr;
     cudaEvent_t ev_h0 = nullptr, ev_h1 = nullptr;   // TB2_TRACE: upload bracket

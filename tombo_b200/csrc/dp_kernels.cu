@@ -1,4 +1,4 @@
-// dp_kernels.cu -- banded DP kernels (sm_100a) and their C-ABI entry points.
+// dp_kernels.cu -- banded DP kernels (sm_90a) and their C-ABI entry points.
 #include "kernels.h"
 #include <algorithm>
 #include <cstdlib>
@@ -22,9 +22,8 @@ int tb2_launch_align(tb2_ctx *ctx, const AlignBatch &b, const AlignLaunchCfg &cf
         smem = smem_of(cfg.smem_cells);
     }
     // resident CTAs per SM: 8 for the static-band kernel (64 registers), 4 for the general
-    // one (128 registers; a 5-CTA build with 102 registers measured 5 % / 14 % slower on the
-    // configs[2] mix / configs[4], profiles/README.md).  228 KB of shared memory per SM, 1 KB
-    // of it reserved per CTA.
+    // one (128 registers; a 5-CTA build with 102 registers was slower on the configs[2] mix
+    // and configs[4]).  228 KB of shared memory per SM (H100), 1 KB of it reserved per CTA.
     const int max_blocks = cfg.klass == 1 ? 8 : 4;
     int blocks_per_sm = (int)std::max<size_t>(1, std::min<size_t>(max_blocks, (228 * 1024) / (smem + 1024)));
     int grid = ctx->sm_count * blocks_per_sm;

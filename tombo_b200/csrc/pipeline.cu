@@ -587,7 +587,7 @@ static int batch_download_impl(tb2_ctx *ctx, int64_t *segs, int64_t *read_start_
 // Chunk schedule of the pipelined batch call (host only).  U = one read per resident DP
 // warp of the lean kernel.  Up to 6 U reads go as one batch (returns 1 chunk); larger
 // batches start with short chunks (the first upload is the only exposed one), continue
-// with chunks of 6 U (measured best of 6 / 8 / 12 on configs[1]) and end with the remainder.
+// with chunks of 6 U (the best of 6 / 8 / 12 on configs[1]) and end with the remainder.
 static std::vector<int64_t> pipeline_chunk_starts(int sm_count, int64_t n_reads)
 {
     std::vector<int64_t> cs;
@@ -690,7 +690,7 @@ static int resquiggle_batch_impl(tb2_ctx *ctx, int64_t n_reads, const void *raw,
     const double t00 = now_ms();
     // (One host thread drives both lanes.  A thread per lane -- kernels of two chunks resident
     // side by side, optionally with the persistent DP grids sized to half an SM each -- was
-    // measured 8-10 % slower end to end on configs[1], profiles/README.md call O: the long
+    // slower end to end on configs[1]: the long
     // persistent DP kernels of one lane stall the short kernels of the other, and nothing is
     // gained back because the device is already never idle in this schedule.)
     rc = upload(0);

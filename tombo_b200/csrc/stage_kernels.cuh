@@ -1,6 +1,6 @@
 // stage_kernels.cuh -- (device code; stage_kernels.cu holds the launch wrappers; tests/emul
 // runs this file on the host)  the non-DP stages of resquiggle_read as batched kernels
-// (sm_100a): signal conversion + k-mer lookup, normalisation, changepoint
+// (sm_90a): signal conversion + k-mer lookup, normalisation, changepoint
 // detection, event means, skipped-base raw-signal DP, base means, Theil-Sen
 // rescaling, final scoring.  One CTA (or warp) per read; arithmetic follows the
 // reference operation for operation (see DESIGN.md "Arithmetic contract").

@@ -1,4 +1,4 @@
-"""``tombo.resquiggle`` per-read API (resquiggle.py:345-1214) on the B200: same
+"""``tombo.resquiggle`` per-read API (resquiggle.py:345-1214) on the GPU: same
 function names, arguments and return namedtuples as the reference; every function
 is a batch of one over the batched C ABI, plus the batched entry point
 :func:`resquiggle_reads` that the throughput numbers are quoted on (per-read
