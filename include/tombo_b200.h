@@ -109,7 +109,9 @@ int64_t tb2_launch_count(tb2_ctx *ctx);
 /* device time (ms, CUDA events on the ctx stream) of the last tb2_batch_compute:
  * out[0] whole compute stage, out[1] sum over launches of the dominant kernel
  * (banded DP, k_align), out[2] number of k_align launches, out[3] reads
- * processed summed over those launches */
+ * processed summed over those launches.  After tb2_group_reg_stats / tb2_reads_ref_levels:
+ * out[0] is the device time from the call's first kernel to its last (upload and download
+ * excluded), out[1..3] are 0 */
 int tb2_last_timing(tb2_ctx *ctx, double *out4);
 
 /* page-locked host buffers (optional; any host memory is accepted by all calls) */
@@ -368,6 +370,46 @@ int tb2_de_novo_read_stats_batch(tb2_ctx *ctx, int64_t n_reads, const double *no
                                  const int64_t *seq_off, const int64_t *read_start,
                                  int64_t fm_offset, double *pvals_out, int64_t *pos_out,
                                  int64_t *stat_off);
+
+/* ---- level_sample_compare and control-sample reference levels ------------------------
+ * One region [reg_start, reg_start + reg_len) per call, already widened by fm_offset
+ * (tombo_stats.py:4337-4342, :3639-3641).  Each sample is a set of ragged per-read level
+ * arrays in genome order: read r has levels[off[r] .. off[r+1]) at genome positions
+ * start[r], start[r] + 1, ... (minus-strand reads reversed by the caller, as
+ * get_single_slot_genome_centric does).  Levels outside the region are ignored; NaN is
+ * missing.  reg_len is at most 2^24, each sample at most 2^30 - 1 reads.
+ *
+ * tb2_group_reg_stats: compute_group_reg_stats :4335-4393.  test 0 = KS (:4236-4255),
+ * 1 = Mann-Whitney U (:4266-4291), 2 = t (:4302-4324); return_stat selects the
+ * *_stat_test variant.  Positions where both samples have >= min_test_reads levels form
+ * runs; runs shorter than 2 fm_offset + 1 are dropped (:4355); with fm_offset > 0 the
+ * p-values of each run go through Fisher's method (calc_window_fishers_method :2252-2271)
+ * and statistics through calc_window_means (:2273-2287), NaN at the first / last fm_offset
+ * positions of a run.  Outputs: covered positions ascending, statistic, sample and control
+ * coverage; *n_out = number of positions (TB2_ERR_CAPACITY when it exceeds cap; the first
+ * cap are written).  U ties: sample levels rank before equal control levels.  Where the
+ * reference raises FloatingPointError (zero pooled variance in the t test, a single level
+ * in each sample) the statistic is NaN.  min_test_reads < 1, reg_len, fm_offset (0 .. 2^24)
+ * or a read count out of range -> TB2_ERR_INVALID_ARG.
+ *
+ * tb2_reads_ref_levels: get_reads_ref :3627-3673.  Per position with >= min_test_reads
+ * levels: np.median (np.mean with est_mean) and np.std of the levels in read order; with
+ * prior_means / prior_sds (reg_len each) compute_posterior_samp_dists' weighted means
+ * (:3589-3594); positions with sd == 0 and uncovered ones are NaN.  cov_out[reg_len] is
+ * the number of levels per position. */
+int tb2_group_reg_stats(tb2_ctx *ctx, int64_t reg_start, int64_t reg_len,
+                        int64_t n_samp, const double *samp_levels, const int64_t *samp_off,
+                        const int64_t *samp_start, int64_t n_ctrl, const double *ctrl_levels,
+                        const int64_t *ctrl_off, const int64_t *ctrl_start, int test,
+                        int return_stat, int64_t min_test_reads, int64_t fm_offset, int64_t cap,
+                        int64_t *pos_out, double *stat_out, int64_t *cov_out,
+                        int64_t *ctrl_cov_out, int64_t *n_out);
+int tb2_reads_ref_levels(tb2_ctx *ctx, int64_t reg_start, int64_t reg_len, int64_t n_reads,
+                         const double *levels, const int64_t *off, const int64_t *start,
+                         int64_t min_test_reads, int est_mean, const double *prior_means,
+                         const double *prior_sds, double mean_prior_weight,
+                         double sd_prior_weight, double *means_out, double *sds_out,
+                         int64_t *cov_out);
 
 #ifdef __cplusplus
 }

@@ -47,4 +47,6 @@ MAX_SCALING_ITERS = 3                      # :171
 MAX_POINTS_FOR_THEIL_SEN = 1000            # :178
 FM_OFFSET_DEFAULT = 1                      # :136
 SMALLEST_PVAL = 1e-50                      # :158
+MEAN_PRIOR_CONST = 5                       # :139
+SD_PRIOR_CONST = 40                        # :140
 COV_DAMP_COUNTS = [2, 0]                   # (unmodified, modified pseudo counts)

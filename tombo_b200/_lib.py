@@ -655,6 +655,49 @@ class Context(object):
                       C.c_int(int(bool(final_clamp))), ptr(out, f64)))
         return out[:means.shape[0]]
 
+    def group_reg_stats(self, reg_start, reg_len, samp, ctrl, test, return_stat, min_test_reads,
+                        fm_offset):
+        """tb2_group_reg_stats.  ``samp`` / ``ctrl`` are ragged genome-ordered reads
+        ``(levels, off, start)``; ``test`` 0 = KS, 1 = U, 2 = t.  Returns a dict of the
+        covered positions (ascending), their statistic and both coverages."""
+        (sl, so, ss), (cl, co, cs) = [(as_f64(l), as_i64(o), as_i64(s)) for l, o, s in (samp, ctrl)]
+        cap = int(reg_len)
+        pos, stat = np.empty(cap, dtype=np.int64), np.empty(cap)
+        cov, ccov = np.empty(cap, dtype=np.int64), np.empty(cap, dtype=np.int64)
+        n = i64(0)
+        fn = self.lib.tb2_group_reg_stats
+        fn.restype = C.c_int
+        self.check(fn(self.handle, i64(int(reg_start)), i64(cap), i64(so.shape[0] - 1),
+                      ptr(sl, f64), ptr(so, i64), ptr(ss, i64), i64(co.shape[0] - 1),
+                      ptr(cl, f64), ptr(co, i64), ptr(cs, i64), C.c_int(int(test)),
+                      C.c_int(int(bool(return_stat))), i64(int(min_test_reads)),
+                      i64(int(fm_offset)), i64(cap), ptr(pos, i64), ptr(stat, f64),
+                      ptr(cov, i64), ptr(ccov, i64), C.byref(n)))
+        m = int(n.value)
+        return dict(pos=pos[:m].copy(), stat=stat[:m].copy(), cov=cov[:m].copy(),
+                    ctrl_cov=ccov[:m].copy())
+
+    def reads_ref_levels(self, reg_start, reg_len, reads, min_test_reads, est_mean=False,
+                         prior_means=None, prior_sds=None, prior_weights=(0.0, 0.0)):
+        """tb2_reads_ref_levels -> (means, sds, cov), each reg_len long"""
+        lv, off, st = as_f64(reads[0]), as_i64(reads[1]), as_i64(reads[2])
+        n = int(reg_len)
+        means, sds, cov = np.empty(n), np.empty(n), np.empty(n, dtype=np.int64)
+        pm = ps = None
+        if prior_means is not None:
+            prior_means, prior_sds = as_f64(prior_means), as_f64(prior_sds)
+            if prior_means.shape[0] != n or prior_sds.shape[0] != n:
+                raise ValueError('prior levels must cover the region')
+            pm, ps = ptr(prior_means, f64), ptr(prior_sds, f64)
+        fn = self.lib.tb2_reads_ref_levels
+        fn.restype = C.c_int
+        self.check(fn(self.handle, i64(int(reg_start)), i64(n), i64(off.shape[0] - 1),
+                      ptr(lv, f64), ptr(off, i64), ptr(st, i64), i64(int(min_test_reads)),
+                      C.c_int(int(bool(est_mean))), pm, ps, f64(float(prior_weights[0])),
+                      f64(float(prior_weights[1])), ptr(means, f64), ptr(sds, f64),
+                      ptr(cov, i64)))
+        return means, sds, cov
+
     def de_novo_read_stats_batch(self, norm_mean, mean_off, seq, seq_off, read_start, fm_offset=1):
         norm_mean, mean_off = as_f64(norm_mean), as_i64(mean_off)
         seq = np.ascontiguousarray(seq, dtype=np.uint8)

@@ -60,7 +60,7 @@ struct tb2_ctx {
     int kmer_width = 0, central_pos = 0, alt_kmer_width = 0;
     // generic scratch pool (named slots), grow-only
     // slots: 0-11 mirror calls, 12-49 batch arrays (pipeline.cu), 50-69 llr.cu,
-    // 70-79 per-warp scratch pools, 80-109 region_stats.cu
+    // 70-79 per-warp scratch pools, 80-109 region_stats.cu, 110-124 group_stats.cu
     std::vector<DevBuf> pool = std::vector<DevBuf>(128);
     // pinned host staging for small results
     void *pinned = nullptr;

@@ -17,7 +17,8 @@ from ._default_parameters import DNA_SAMP_TYPE, RNA_SAMP_TYPE  # noqa: F401
 __all__ = [
     'TomboError', 'readData', 'TomboMotif', 'resquiggleParams', 'startClipParams',
     'stallParams', 'resquiggleResults', 'alignInfo', 'genomeLocation', 'sequenceData',
-    'channelInfo', 'dpResults', 'scaleValues', 'seqSampleType', 'regionStats', 'get_seq_kmers',
+    'channelInfo', 'dpResults', 'scaleValues', 'seqSampleType', 'regionStats', 'groupStats',
+    'get_seq_kmers', 'rev_comp',
     'valid_cpts_w_cap', 'valid_cpts_w_cap_t_test', 'banded_traceback',
     'adaptive_banded_forward_pass', 'get_raw_read_slot', 'get_multiple_slots_read_centric']
 
@@ -26,6 +27,7 @@ SINGLE_LETTER_CODE = {
     'K': '[GT]', 'M': '[AC]', 'N': '[ACGT]', 'R': '[AG]', 'S': '[CG]', 'V': '[ACG]',
     'W': '[AT]', 'Y': '[CT]'}
 INVALID_BASES = re.compile('[^ACGT]')
+INVALID_BASE_RUNS = re.compile('[^ACGT]+')
 
 
 class TomboError(Exception):
@@ -117,6 +119,11 @@ class regionStats(namedtuple('regionStats', (
     """Region statistics (tombo_helper.py:299-313)"""
 
 
+class groupStats(namedtuple('groupStats', (
+        'reg_stats', 'reg_poss', 'chrm', 'strand', 'start', 'reg_cov', 'ctrl_cov'))):
+    """Level-comparison region statistics (tombo_helper.py:315-328)"""
+
+
 class seqSampleType(namedtuple('seqSampleType', ('name', 'rev_sig'))):
     """tombo_helper.py:330"""
 
@@ -131,6 +138,12 @@ def get_seq_kmers(seq, kmer_width, rev_strand=False):
 
 
 _COMP = {'A': 'T', 'C': 'G', 'G': 'C', 'T': 'A', '[': ']', ']': '['}
+_COMP_BASES = dict(zip(map(ord, 'ACGT'), map(ord, 'TGCA')))
+
+
+def rev_comp(seq):
+    """tombo_helper.py:375-378 (other characters are kept as they are)"""
+    return seq.translate(_COMP_BASES)[::-1]
 
 
 class TomboMotif(object):

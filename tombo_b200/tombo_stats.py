@@ -13,7 +13,7 @@ from . import tombo_helper as th
 from ._default_parameters import (
     ALGN_PARAMS_TABLE, SEG_PARAMS_TABLE, RNA_SAMP_TYPE, DNA_SAMP_TYPE,
     MIN_EVENT_TO_SEQ_RATIO, OCLLHR_SCALE, OCLLHR_HEIGHT, OCLLHR_POWER, STALL_PARAMS,
-    FM_OFFSET_DEFAULT, SMALLEST_PVAL)
+    FM_OFFSET_DEFAULT, SMALLEST_PVAL, MEAN_PRIOR_CONST, SD_PRIOR_CONST)
 
 __all__ = [
     'TomboModel', 'AltModel', 'normalize_raw_signal', 'compute_base_means',
@@ -21,7 +21,9 @@ __all__ = [
     'compute_num_events', 'get_dynamic_prog_params', 'identify_stalls',
     'compute_alt_model_read_stats', 'trim_seq_and_means', 'apply_per_read_thresh',
     'collate_reg_stats', 'calc_damp_fraction', 'calc_window_fishers_method',
-    'compute_de_novo_read_stats', 'compute_sample_compare_read_stats']
+    'compute_de_novo_read_stats', 'compute_sample_compare_read_stats',
+    'compute_ks_tests', 'compute_u_tests', 'compute_t_tests', 'calc_window_means',
+    'compute_group_reg_stats', 'get_reads_ref', 'compute_posterior_samp_dists']
 
 # E|N(0,1)| = sqrt(2 / pi); the reference evaluates scipy.stats.halfnorm.expect()
 # (tombo_stats.py:84), which returns this value (SURVEY.md 8c-2)
@@ -29,6 +31,10 @@ HALF_NORM_EXPECTED_VAL = float(np.sqrt(2.0 / np.pi))
 STANDARD_MODEL_NAME = 'standard'
 CONST_SD_MODEL = True                     # tombo_stats.py:112
 SAMP_COMP_TXT, DE_NOVO_TXT, ALT_MODEL_TXT = 'sample_compare', 'de_novo', 'model_compare'   # :89-91
+KS_TEST_TXT, U_TEST_TXT, T_TEST_TXT = 'ks_test', 'u_test', 't_test'                  # :95-97
+KS_STAT_TEST_TXT, U_STAT_TEST_TXT, T_STAT_TEST_TXT = 'ks_stat_test', 'u_stat_test', 't_stat_test'
+LEVEL_STATS_TXTS = (KS_TEST_TXT, U_TEST_TXT, T_TEST_TXT,
+                    KS_STAT_TEST_TXT, U_STAT_TEST_TXT, T_STAT_TEST_TXT)               # :101-103
 NORM_TYPES = ('none', 'pA', 'pA_raw', 'median', 'robust_median', 'median_const_scale')
 _CODE = {'A': 0, 'C': 1, 'G': 2, 'T': 3}
 
@@ -101,6 +107,24 @@ class TomboModel(object):
             ref_sds = np.array([self.sds[kmer] for kmer in seq_kmers])
         except KeyError:
             raise th.TomboError('Invalid sequence encountered from genome sequence.')
+        return ref_means, ref_sds
+
+    def get_exp_levels_from_seq_with_gaps(self, reg_seq, rev_strand):
+        """tombo_stats.py:886-918: expected levels of every k-mer of ``reg_seq``; NaN for
+        k-mers that touch a non-ACGT base"""
+        n = len(reg_seq) - self.kmer_width + 1
+        ref_means, ref_sds = np.full(n, np.nan), np.full(n, np.nan)
+        prev = 0
+        for m in list(th.INVALID_BASE_RUNS.finditer(reg_seq)) + [None]:
+            stop = len(reg_seq) if m is None else m.start()
+            if stop - prev >= self.kmer_width:
+                sm, ss = self.get_exp_levels_from_seq(reg_seq[prev:stop])
+                ref_means[prev:stop - self.kmer_width + 1] = sm
+                ref_sds[prev:stop - self.kmer_width + 1] = ss
+            if m is not None:
+                prev = m.end()
+        if rev_strand:
+            ref_means, ref_sds = ref_means[::-1], ref_sds[::-1]
         return ref_means, ref_sds
 
 
@@ -549,3 +573,148 @@ def compute_sample_compare_read_stats(r_data, ctrl_means, ctrl_sds, fm_offset=FM
         np.ascontiguousarray(r_means), cm, cs, np.array([0, r_means.shape[0]]), fm_offset, False)
     r_poss = np.where(~np.isnan(r_pvals))[0]
     return {SAMP_COMP_TXT: r_pvals[r_poss]}, {SAMP_COMP_TXT: r_poss + read_start}, read_id
+
+
+# ---------------------------------------------------------------------------
+# level_sample_compare and control-sample reference levels (tombo_stats.py:2273-2287,
+# 3572-3673, 4236-4393)
+# ---------------------------------------------------------------------------
+_LEVEL_TESTS = {KS_TEST_TXT: (0, False), U_TEST_TXT: (1, False), T_TEST_TXT: (2, False),
+                KS_STAT_TEST_TXT: (0, True), U_STAT_TEST_TXT: (1, True),
+                T_STAT_TEST_TXT: (2, True)}
+
+
+def _ragged_reads(base_levels, reg_start):
+    """positions x reads level matrix (``intervalData.get_base_levels``) -> ragged
+    genome-ordered reads ``(levels, off, start)``: each column from its first to its last
+    non-NaN level, in column (read) order"""
+    bl = np.asarray(base_levels, dtype=np.float64)
+    if bl.ndim != 2:
+        raise th.TomboError('Base levels must be a positions x reads matrix.')
+    valid = ~np.isnan(bl)
+    cols = np.nonzero(valid.any(axis=0))[0]
+    first = valid.argmax(axis=0)[cols]
+    last = bl.shape[0] - valid[::-1].argmax(axis=0)[cols]
+    lens = (last - first).astype(np.int64)
+    levels = (np.concatenate([bl[f:l, c] for c, f, l in zip(cols, first, last)])
+              if cols.shape[0] else np.zeros(0))
+    off = np.concatenate([[0], np.cumsum(lens)]).astype(np.int64)
+    return levels, off, (reg_start + first).astype(np.int64)
+
+
+def _widened_levels(reg_data, fm_offset):
+    return reg_data.copy().update(start=reg_data.start - fm_offset,
+                                  end=reg_data.end + fm_offset).get_base_levels()
+
+
+def _dense_level_tests(samp_base_levels, ctrl_base_levels, return_stat, test):
+    samp = np.asarray(samp_base_levels, dtype=np.float64)
+    ctrl = np.asarray(ctrl_base_levels, dtype=np.float64)
+    n = samp.shape[0]
+    out = np.full(n, np.nan)
+    if n == 0:
+        return out
+    r = _lib.get_context().group_reg_stats(
+        0, n, _ragged_reads(samp, 0), _ragged_reads(ctrl, 0), test, return_stat, 1, 0)
+    out[r['pos']] = r['stat']
+    return out
+
+
+def compute_ks_tests(samp_base_levels, ctrl_base_levels, return_stat):
+    """tombo_stats.py:4236-4260 on positions x reads matrices (NaN = missing).  A position
+    where either sample has no level is NaN (the reference raises FloatingPointError)."""
+    return _dense_level_tests(samp_base_levels, ctrl_base_levels, return_stat, 0)
+
+
+def compute_u_tests(samp_base_levels, ctrl_base_levels, return_stat):
+    """tombo_stats.py:4262-4297.  Tied levels: a sample level ranks before an equal
+    control level (the reference's unstable argsort leaves that order undefined)."""
+    return _dense_level_tests(samp_base_levels, ctrl_base_levels, return_stat, 1)
+
+
+def compute_t_tests(samp_base_levels, ctrl_base_levels, return_stat):
+    """tombo_stats.py:4299-4333.  Zero pooled variance, or one level in each sample, gives
+    NaN (the reference raises FloatingPointError)."""
+    return _dense_level_tests(samp_base_levels, ctrl_base_levels, return_stat, 2)
+
+
+def calc_window_means(stats, lag):
+    """tombo_stats.py:2273-2287 (host numpy, as in the reference; compute_group_reg_stats
+    applies the same window on the device)"""
+    assert lag > 0, 'Invalid window provided.'
+    width = (lag * 2) + 1
+    if stats.shape[-1] < width:
+        raise th.TomboError("Statistics vector too short for window mean compuation.")
+    m_stats = np.full(stats.shape, np.nan)
+    m_stats[..., lag:-lag] = np.mean(np.lib.stride_tricks.sliding_window_view(
+        stats, width, axis=-1), -1)
+    return m_stats
+
+
+def compute_group_reg_stats(reg_data, ctrl_reg_data, fm_offset, min_test_reads, stat_type):
+    """tombo_stats.py:4335-4393 -> ``[(stat_type, tombo_helper.groupStats)]`` or ``[]``.
+    Base levels come from ``reg_data.copy().update(...).get_base_levels()``; coverage, runs,
+    the per-position test and the window all run on the device in one call.  The widened
+    region holds at most 2^24 positions and each sample at most 2^30 - 1 reads (larger
+    inputs raise ``_lib.TomboB200Error``); ``fm_offset`` has no other limit."""
+    if stat_type not in _LEVEL_TESTS:
+        raise NotImplementedError('Unrecognized test type.')
+    test, return_stat = _LEVEL_TESTS[stat_type]
+    start = reg_data.start - fm_offset
+    size = reg_data.end - reg_data.start + 2 * fm_offset
+    samp = _ragged_reads(_widened_levels(reg_data, fm_offset), start)
+    ctrl = _ragged_reads(_widened_levels(ctrl_reg_data, fm_offset), start)
+    r = _lib.get_context().group_reg_stats(start, size, samp, ctrl, test, return_stat,
+                                           min_test_reads, fm_offset)
+    if r['pos'].shape[0] == 0:
+        return []
+    return [(stat_type, th.groupStats(r['stat'], r['pos'], reg_data.chrm, reg_data.strand,
+                                      reg_data.start, r['cov'], r['ctrl_cov']))]
+
+
+def _prior_levels(ctrl_reg_data, std_ref, fm_offset):
+    """compute_posterior_samp_dists :3575-3587: expected levels over the widened region"""
+    dnstrm_bases = std_ref.kmer_width - std_ref.central_pos - 1
+    plus = ctrl_reg_data.strand == '+'
+    begin_lag = std_ref.central_pos if plus else dnstrm_bases
+    end_lag = dnstrm_bases if plus else std_ref.central_pos
+    reg_seq = ctrl_reg_data.copy().update(
+        start=ctrl_reg_data.start - begin_lag - fm_offset,
+        end=ctrl_reg_data.end + end_lag + fm_offset).add_seq().seq
+    if ctrl_reg_data.strand == '-':
+        reg_seq = th.rev_comp(reg_seq)
+    return std_ref.get_exp_levels_from_seq_with_gaps(reg_seq, ctrl_reg_data.strand == '-')
+
+
+def compute_posterior_samp_dists(ctrl_means, ctrl_sds, ctrl_cov, ctrl_reg_data, std_ref,
+                                 prior_weights, min_test_reads, fm_offset):
+    """tombo_stats.py:3572-3625: weighted means of the control levels and the model's
+    expected levels (elementwise host numpy, as in the reference; get_reads_ref applies
+    the same weights on the device)"""
+    reg_ref_means, reg_ref_sds = _prior_levels(ctrl_reg_data, std_ref, fm_offset)
+    post_ref_means = (((prior_weights[0] * reg_ref_means) + (ctrl_cov * ctrl_means)) /
+                      (prior_weights[0] + ctrl_cov))
+    post_ref_sds = (((prior_weights[1] * reg_ref_sds) + (ctrl_cov * ctrl_sds)) /
+                    (prior_weights[1] + ctrl_cov))
+    return post_ref_means, post_ref_sds
+
+
+def get_reads_ref(reg_data, min_test_reads, fm_offset, std_ref=None, prior_weights=None,
+                  est_mean=False):
+    """tombo_stats.py:3627-3673 -> (means, sds, {position: coverage}).  Median (or mean)
+    and standard deviation of the levels per position, the optional posterior with the
+    model's expected levels, and the sd == 0 mask run on the device in one call.  The
+    widened region holds at most 2^24 positions and at most 2^30 - 1 reads."""
+    start = reg_data.start - fm_offset
+    size = reg_data.end - reg_data.start + 2 * fm_offset
+    reads = _ragged_reads(_widened_levels(reg_data, fm_offset), start)
+    pm = ps = None
+    weights = (0.0, 0.0)
+    if std_ref is not None:
+        weights = (MEAN_PRIOR_CONST, SD_PRIOR_CONST) if prior_weights is None else prior_weights
+        pm, ps = _prior_levels(reg_data, std_ref, fm_offset)
+    means, sds, cov = _lib.get_context().reads_ref_levels(
+        start, size, reads, min_test_reads, est_mean, pm, ps, weights)
+    if not (cov >= min_test_reads).any():
+        return np.full(size, np.nan), np.full(size, np.nan), {}
+    return means, sds, dict(zip(range(start, start + size), cov))
