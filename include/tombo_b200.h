@@ -219,8 +219,10 @@ int tb2_debug_last_assignment(tb2_ctx *ctx, int64_t n_bases, int64_t *starts_out
  * pairs where the reciprocal-based division of the DP rows differs from a / b */
 int tb2_debug_div_check(tb2_ctx *ctx, uint64_t seed, int blocks, int per_thread,
                         uint64_t *mismatches, double *example4);
-/* tuning / test counters: [0] Theil-Sen calls, [1] fp32-bracket path, [2] exact
- * histogram path, [3] generic radix-select path */
+/* tuning / test counters (device-global, cumulative: compare deltas): [0] Theil-Sen calls,
+ * [1] fp32 bracket over every pair, [2] exact histogram path, [3] generic radix-select path,
+ * [4] fp32 bracket over sampled pairs, [5] sort-and-sweep finished, [6] sort-and-sweep
+ * abandoned (one of [1]-[4] then finishes), [7] sweep phases (TS_DEBUG builds only) */
 int tb2_debug_counters(tb2_ctx *ctx, unsigned long long *out8, int reset);
 /* resolve_skipped_bases_with_raw resquiggle.py:402-540 */
 int tb2_resolve_skipped_bases_with_raw(

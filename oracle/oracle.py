@@ -120,6 +120,12 @@ def np_mean(x):
     return lib().orc_np_mean(px, i64(x.shape[0]))
 
 
+def perm_index(i, n, key):
+    """Keyed bijection on [0, n): the Theil-Sen sub-sample index i (stands in for
+    np.random.choice(n, 1000, replace=False), tombo_stats.py:411-416)."""
+    return int(lib().orc_perm_index(i64(i), i64(n), C.c_uint32(key)))
+
+
 def linspace(start, stop, num):
     out = np.empty(max(num, 0))
     lib().orc_linspace(f64(start), f64(stop), i64(num), out.ctypes.data_as(P(f64)))

@@ -70,7 +70,7 @@ def test_theil_sen_matches_oracle(orc, dna_model, RPcls, nb, seed):
     bm = orc.new_means(nsig, seg2)
     s1, o1 = orc.theil_sen(sv[0], sv[1], bm, rm, key=77)
     s2, o2 = emul.theil_sen(sv[0], sv[1], bm, rm, key=77)
-    assert s1 == s2 and o1[:2] == o2[:2]
+    assert s1 == s2 and o1 == o2
 
 
 def test_theil_sen_adversarial_inputs_match_oracle(orc):
@@ -100,7 +100,7 @@ def test_theil_sen_adversarial_inputs_match_oracle(orc):
         s2, o2 = emul.theil_sen(0.3, 1.7, ev, md, key=9)
         assert s1 == s2, (it, n, kind)
         if s1 == 0:
-            assert o1[:2] == o2[:2], (it, n, kind)
+            assert o1 == o2, (it, n, kind)
 
 
 def test_block_select_on_integer_and_tied_values():
@@ -152,7 +152,7 @@ def test_theil_sen_equal_levels_stay_on_the_sort_and_sweep_path(orc):
         s2, o2 = emul.theil_sen(0.1, 1.2, bm, rm, key=3)
         assert s1 == s2, (it, n)
         if s1 == 0:
-            assert o1[:2] == o2[:2], (it, n, o1, o2)
+            assert o1 == o2, (it, n, o1, o2)
             n_cases += 1
     L.emul_ts_counters(out, 0)
     c = list(out)

@@ -116,13 +116,25 @@ def test_theil_sen_bit_exact(ctx, orc, n, seed):
 
 
 def test_theil_sen_heavy_tail_uses_exact_fallback(ctx, orc):
+    from test_theil_sen_gpu import debug_counters
+    import theil_sen_cases as tc
     rs = np.random.RandomState(9)
     n = 300
     md = rs.normal(0, 1.4826, n)
-    ev = rs.standard_cauchy(n)        # slopes all over the place
+    ev = rs.standard_cauchy(n)        # slopes all over the place: sort-and-sweep still copes
     s0, o0 = orc.theil_sen(0.0, 1.0, ev, md, 0)
     s1, o1 = ctx.theil_sen(0.0, 1.0, ev, md, 0)
     assert s0 == s1 == 0 and o0 == o1
+    # Cauchy event means on a line to 1e-9: every gap is inside the guards, so sort-and-sweep
+    # is abandoned and the exact 2048-bin histogram over all pairs finishes
+    md = ev + 1e-9 * rs.normal(0, 1, n)
+    before = debug_counters(ctx)
+    s1, o1 = ctx.theil_sen(0.0, 1.0, ev, md, 0)
+    delta = debug_counters(ctx) - before
+    s0, o0 = orc.theil_sen(0.0, 1.0, ev, md, 0)
+    assert s0 == s1 == 0 and o0 == o1
+    assert delta[tc.READS] == 1 and delta[tc.SWEEP_ABANDONED] == 1 and delta[tc.HISTOGRAM] == 1, delta
+    assert delta[tc.SWEEP] == delta[tc.FP32_ALL] == delta[tc.FP32_SAMPLED] == delta[tc.GENERIC] == 0, delta
 
 
 def test_resolve_skipped_bases_bit_exact(ctx, orc, RPcls):

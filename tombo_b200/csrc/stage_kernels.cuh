@@ -933,8 +933,10 @@ __global__ void __launch_bounds__(ST_THREADS) k_base_means(BatchView b)
 // 2048-bin histogram over a sample-derived bracket narrows the median to one
 // bin, whose members are selected exactly (generic radix select as fall-back).
 // ===========================================================================
-// debug counters (tests / tuning): [0] Theil-Sen reads, [1] fast path, [2] exact
-// histogram path, [3] generic select path, [5] sort-and-sweep path, [6] ... abandoned
+// debug counters (tests / tuning): [0] Theil-Sen reads, [1] fp32 bracket over every pair,
+// [2] exact histogram path, [3] generic select path, [4] fp32 bracket over sampled pairs,
+// [5] sort-and-sweep finished, [6] sort-and-sweep abandoned (one of [1]-[4] then finishes),
+// [7] odd-even sweep phases (TS_DEBUG builds only)
 __device__ unsigned long long g_tb2_counters[8];
 
 #define TS_MAX 1000
