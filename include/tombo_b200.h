@@ -359,7 +359,10 @@ int tb2_region_stats_finalize(tb2_ctx *ctx, double unmod_count, double mod_count
  * np.maximum(p, SMALLEST_PVAL)).  Outputs have the inputs' length; the first / last
  * fm_offset entries of a segment and entries with NaN inputs are NaN.  With ref_means and
  * ref_sds both NULL, `means` holds p-values already (the bare Fisher window).  Floating point:
- * erfc / log / exp of the device library, parity with scipy within rtol 1e-7.
+ * erfc / log of the device library and tb2_chi2_sf_even (special.cuh: the closed form below
+ * y = 700, Loader's saddle-point form above, relative error <= 1e-12 + 16 u y); each p within
+ * (4 x^2 + 16) u of the exact value (x = z / sqrt 2, u = 2^-53), each window within the
+ * propagated log-sum error plus the chi-square error (tests/stats_cases.py).
  * tb2_de_novo_read_stats_batch runs the de novo test for whole '+' strand reads with
  * the canonical levels looked up on the device (tb2_set_model): stat_off (n_reads + 1,
  * filled) counts n_bases - (kmer_width - 1) positions per read. */

@@ -4,6 +4,7 @@ import numpy as np
 import pytest
 
 import golden_util as gu
+import stats_cases as sc
 
 pytestmark = pytest.mark.gpu
 
@@ -171,8 +172,10 @@ def test_compute_alt_model_read_stats_matches_reference():
                                                           use_standard_llhr=True)
         a, b = int(g['site_off'][i]), int(g['site_off'][i + 1])
         assert np.array_equal(pos['5mC'], g['pos'][a:b])
-        np.testing.assert_allclose(llr['5mC'], g['llr_scaled'][a:b], rtol=1e-5, atol=1e-5)
-        np.testing.assert_allclose(llr_s['5mC'], g['llr_standard'][a:b], rtol=1e-5, atol=1e-5)
+        assert np.array_equal(llr_s['5mC'], g['llr_standard'][a:b])
+        _, _, _, s_abs = sc.llr_of_genome_read(norm_mean, res.genome_seq, 1000 * i, kmer_ref,
+                                               cpos, 0)
+        sc.assert_llr(llr['5mC'], g['llr_scaled'][a:b], s_abs, 0, len(kmer_ref[0][0]))
 
 
 def test_identify_stalls_matches_oracle(orc):

@@ -1,5 +1,6 @@
 """The numpy / scipy restatement that the level-test GPU sweeps compare against reproduces
 the unmodified reference's goldens (tests/golden/group_stats.npz) without a GPU."""
+import math
 import os
 import sys
 
@@ -54,6 +55,7 @@ def _special_lib():
     lib = C.CDLL(path)
     for name, args in (('tb2_host_kolmogorov_sf', [C.c_double]),
                        ('tb2_host_t_two_sided_p', [C.c_double, C.c_double]),
+                       ('tb2_host_chi2_sf_even', [C.c_double, C.c_int]),
                        ('tb2_host_div12', [C.c_uint64, C.c_uint64])):
         getattr(lib, name).restype = C.c_double
         getattr(lib, name).argtypes = args
@@ -99,6 +101,46 @@ def test_student_t_matches_scipy_on_a_dense_grid():
             want[i] = float(mpmath.betainc(mpmath.mpf(df) / 2, 0.5, 0, x, regularized=True))
         worst = max(worst, _rel_err(got, want))
     assert worst <= 1e-9, worst
+
+
+def _old_chi2_sf_even(y, k):
+    """the closed form exactly as the kernels evaluated it before the large-y branch"""
+    term, s = 1.0, 1.0
+    for i in range(1, k):
+        term *= y / float(i)
+        s += term
+    return math.exp(-y) * s
+
+
+def test_chi2_sf_even_matches_mpmath_on_every_window_width():
+    """Q(k, y) = chi2.sf(2 y, 2 k) for every de novo / sample-compare width k = 1..129 and
+    the widths of fm_offset up to 2^24, with y up to the width's maximum (every p at the
+    1e-50 clamp, y = 115.13 k) and dense where the closed form hands over (700..750)."""
+    import stats_cases as sc
+    lib = _special_lib()
+    ks = list(range(1, 130)) + [681, 701, 721, 801, 2001, 2 ** 15 + 1, 2 ** 20 + 1, 2 ** 25 + 1]
+    worst, n_tiny, n_close = 0.0, 0, 0
+    for k in ks:
+        ymax = sc.Y_PER_CLAMPED_P * k
+        ys = np.concatenate([np.linspace(0.0, ymax, 25), np.linspace(700.0, 750.0, 26),
+                             [k - 1.0, float(k), k + 0.5, np.nextafter(700.0, 0.0)]])
+        for y in np.unique(ys[ys <= ymax]):
+            y = float(y)
+            got = lib.tb2_host_chi2_sf_even(y, k)
+            assert not math.isnan(got), (k, y)
+            if y < 700.0 and k <= 2001:
+                # unchanged below 700: same operations, same bits
+                assert got == _old_chi2_sf_even(y, k), (k, y)
+            want = sc.exact_chi2_sf_even(y, k)
+            if want > 1e-300:
+                err = abs(got - float(want)) / float(want)
+                worst = max(worst, err / sc.chi2_bound(y))
+                n_close += 1
+            else:
+                assert got <= 1e-300, (k, y, got)
+                n_tiny += 1
+    assert worst <= 1.0, worst
+    assert n_close > 2000 and n_tiny > 1000
 
 
 def test_div12_rounds_like_python():

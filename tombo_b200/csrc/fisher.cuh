@@ -3,6 +3,7 @@
 // (region_stats.cu) and the per-position level tests (group_stats.cu).
 #pragma once
 #include <cmath>
+#include "special.cuh"
 
 namespace {
 // One block per segment (a read, or a run of covered positions); `out` has the segment's
@@ -16,14 +17,6 @@ __device__ __forceinline__ double two_sided_p(double m, double rm, double rs)
 __device__ __forceinline__ double np_maximum(double a, double b)   // NaN propagates
 {
     return (a != a) ? a : (a < b ? b : a);
-}
-
-__device__ __forceinline__ double chi2_sf_even(double y, int k)
-{
-    // scipy.stats.chi2.sf(2 y, 2 k) = Q(k, y) = exp(-y) * sum_{i<k} y^i / i!
-    double term = 1.0, sum = 1.0;
-    for (int i = 1; i < k; ++i) { term *= y / (double)i; sum += term; }
-    return exp(-y) * sum;
 }
 
 struct FisherArgs {
@@ -82,7 +75,7 @@ __global__ void __launch_bounds__(256) k_fisher(FisherArgs a)
         if (n >= width && i >= lag && i < n - lag) {
             double s = logp[i - lag];
             for (int j = 1; j < width; ++j) s += logp[i - lag + j];
-            f = (s != s) ? s : chi2_sf_even(-s, width);      // chi2.sf(log_sums * -2, width * 2)
+            f = (s != s) ? s : tb2_chi2_sf_even(-s, width);  // chi2.sf(log_sums * -2, width * 2)
             if (a.final_clamp) f = np_maximum(f, a.smallest);   // :3870-3871 (de novo only)
         }
         out[i] = f;

@@ -141,6 +141,11 @@ extern "C" int tb2_alt_model_llr_batch(tb2_ctx *ctx, int64_t n_reads, const doub
     if (n_reads == 0) return TB2_OK;
     if (!norm_mean || !seq || !llr_out || !pos_out) return TB2_ERR_INVALID_ARG;
     const int n = (int)n_reads;
+    // every read holds nb means and the nb + K - 1 bases of their k-mers
+    for (int r = 0; r < n; ++r) {
+        const long long nb = mean_off[r + 1] - mean_off[r];
+        if (nb < 0 || seq_off[r + 1] - seq_off[r] != nb + (ctx->kmer_width - 1)) return TB2_ERR_INVALID_ARG;
+    }
     auto &P = ctx->pool;
     cudaStream_t s = ctx->stream;
     const size_t tm = (size_t)mean_off[n], ts = (size_t)seq_off[n];

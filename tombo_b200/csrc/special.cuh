@@ -1,7 +1,9 @@
-// special.cuh -- fp64 special functions of the level tests (group_stats.cu), host and device.
+// special.cuh -- fp64 special functions of the level tests (group_stats.cu) and of the Fisher
+// windows (fisher.cuh), host and device.
 //
 //   tb2_kolmogorov_sf(y)      scipy.special.kolmogorov == stats.kstwobign.sf
 //   tb2_t_two_sided_p(df, t)  2 * scipy.special.stdtr(df, t) for t <= 0
+//   tb2_chi2_sf_even(y, k)    scipy.stats.chi2.sf(2 y, 2 k)
 //   tb2_div12(P)              Python's int / 12 (correctly rounded) for a 128-bit P
 #pragma once
 #include <math.h>
@@ -106,6 +108,91 @@ TB2_HD double tb2_t_two_sided_p(double df, double t)
     const double front = exp(tb2_lgamma_half_ratio(a) - 0.57236494292470008707 + a * lx + b * ly);
     if (x < (a + 1.0) / (a + b + 2.0)) return front * tb2_betacf(a, b, x) / a;
     return 1.0 - front * tb2_betacf(b, a, y) / b;
+}
+
+// ---------------------------------------------------------------------------
+// scipy.stats.chi2.sf(2 y, 2 k) = Q(k, y) = exp(-y) * sum_{i<k} y^i / i!, the Poisson
+// probability P(N <= k - 1), N ~ Poisson(y).  Fisher's method over a window of k p-values
+// asks for it with y = -sum log p.
+//
+// y < 700: the closed form, operation for operation.  exp(-y) is a normal double and the sum
+// stays below e^700, so nothing under- or overflows; every term is a product of at most
+// 2 i roundings, so the relative error stays within about 2 (y + 10 sqrt(y)) u.  The loop
+// stops once the terms decrease (i > y) and adding one no longer changes the sum: every
+// later term is smaller still, so the result is the same as summing all k terms.
+//
+// y >= 700: exp(-y) would underflow before the sum makes up for it (and for y beyond ~12 000
+// the sum overflows, 0 * inf = NaN).  Instead the largest term of the sum, j = min(k - 1,
+// floor(y)), is evaluated in logarithms with Loader's saddle-point form
+//   log p(j; y) = -stirlerr(j) - bd0(j, y) - log(2 pi j) / 2,
+// which has no lgamma cancellation at large j, and the other terms are summed outward from it
+// as ratios p(j-1)/p(j) = j / y and p(j+1)/p(j) = y / (j+1) until they are negligible:
+// the terms fall off like a Gaussian of width sqrt(y) around the mode (or geometrically below
+// it), so at most min(k, ~40 sqrt(y)) ratios are taken.  Rounding log p(j; y), whose size is
+// up to ~y, costs ~y u relative after exp; the ratio sum adds a few u per term.
+// ---------------------------------------------------------------------------
+
+// stirlerr(n) = log(n!) - log(sqrt(2 pi n) (n/e)^n) for an integer n >= 1
+TB2_HD double tb2_stirlerr(double n)
+{
+    if (n <= 15.0)
+        return lgamma(n + 1.0) - (n + 0.5) * log(n) + n - 0.91893853320467274178;  // log sqrt(2 pi)
+    const double r = 1.0 / n, r2 = r * r;
+    return r * (1.0 / 12.0 - r2 * (1.0 / 360.0 - r2 * (1.0 / 1260.0 - r2 * (1.0 / 1680.0 -
+                r2 * (1.0 / 1188.0)))));
+}
+
+// bd0(x, m) = x log(x / m) + m - x >= 0, with the series in v = (x - m) / (x + m) where the
+// direct form cancels
+TB2_HD double tb2_bd0(double x, double m)
+{
+    if (fabs(x - m) < 0.1 * (x + m)) {
+        double v = (x - m) / (x + m);
+        double s = (x - m) * v, ej = 2.0 * x * v;
+        v = v * v;
+        for (int j = 1; j < 1000; ++j) {
+            ej *= v;
+            const double s1 = s + ej / (double)(2 * j + 1);
+            if (s1 == s) break;
+            s = s1;
+        }
+        return s;
+    }
+    return x * log(x / m) + m - x;
+}
+
+TB2_HD double tb2_chi2_sf_even(double y, int k)
+{
+    if (y != y) return y;
+    if (y < 700.0) {
+        double term = 1.0, sum = 1.0;
+        for (int i = 1; i < k; ++i) {
+            term *= y / (double)i;
+            const double prev = sum;
+            sum += term;
+            if (sum == prev && (double)i > y) break;
+        }
+        return exp(-y) * sum;
+    }
+    if (isinf(y)) return 0.0;
+    const double jt = fmin((double)(k - 1), floor(y));       // the largest term
+    const double lp = jt == 0.0 ? -y
+                                : -tb2_stirlerr(jt) - tb2_bd0(jt, y) - 0.5 * log(6.283185307179586477 * jt);
+    if (lp < -760.0) return 0.0;                              // Q < e^-740
+    const double eps = 1e-17;
+    double s = 1.0, t = 1.0;
+    for (double j = jt; j >= 1.0; j -= 1.0) {                // p(j - 1) / p(j) = j / y
+        t *= j / y;
+        s += t;
+        if (t < eps * s) break;
+    }
+    t = 1.0;
+    for (double j = jt + 1.0; j <= (double)(k - 1); j += 1.0) {   // p(j) / p(j - 1) = y / j
+        t *= y / j;
+        s += t;
+        if (t < eps * s) break;
+    }
+    return exp(lp) * s;
 }
 
 // p / 12 correctly rounded to double, as Python's int / int evaluates tot * (tot + 1) / 12
