@@ -211,10 +211,6 @@ int tb2_find_seq_start_in_events(tb2_ctx *ctx, const double *event_means,
                                  int64_t num_events, int check_score,
                                  double sig_match_thresh, int64_t *start_loc,
                                  double *events_per_base, int *read_status);
-/* debug aid for parity tests: band event starts (n_bases) and event-space
- * traceback (n_bases + 1) left by the last tb2_find_adaptive_base_assignment */
-int tb2_debug_last_assignment(tb2_ctx *ctx, int64_t n_bases, int64_t *starts_out,
-                              int64_t *read_tb_out);
 /* self-check: blocks x 256 x per_thread random / adversarial (a, b) pairs; counts
  * pairs where the reciprocal-based division of the DP rows differs from a / b */
 int tb2_debug_div_check(tb2_ctx *ctx, uint64_t seed, int blocks, int per_thread,

@@ -44,14 +44,12 @@ extern "C" void tb2_ctx_destroy(tb2_ctx *ctx)
     cudaStreamSynchronize(ctx->stream);
     for (tb2_ctx *ln : ctx->lanes) tb2_ctx_destroy(ln);
     ctx->lanes.clear();
-    for (auto &b : ctx->pool) b.release();
-    ctx->model_means.release(); ctx->model_sds.release(); ctx->alt_means.release();
     if (ctx->pinned) cudaFreeHost(ctx->pinned);
     cudaEventDestroy(ctx->ev0); cudaEventDestroy(ctx->ev1);
     cudaEventDestroy(ctx->ev2); cudaEventDestroy(ctx->ev3);
     if (ctx->ev_t0) { cudaEventDestroy(ctx->ev_t0); cudaEventDestroy(ctx->ev_t1); }
     cudaStreamDestroy(ctx->stream);
-    delete ctx;
+    delete ctx;   // the DevBuf destructors free the model tables and every module's buffers
 }
 
 extern "C" const char *tb2_last_error(tb2_ctx *ctx) { return ctx ? ctx->err.c_str() : "null ctx"; }

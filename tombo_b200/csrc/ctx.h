@@ -9,10 +9,14 @@
 #include <vector>
 #include "../../include/tombo_b200.h"
 
+// grow-only device buffer; frees what it owns when destroyed
 struct DevBuf {
     void *p = nullptr;
     size_t cap = 0;
-    // grow-only device buffer
+    DevBuf() = default;
+    DevBuf(const DevBuf &) = delete;
+    DevBuf &operator=(const DevBuf &) = delete;
+    ~DevBuf() { release(); }
     cudaError_t reserve(size_t bytes)
     {
         if (bytes <= cap) return cudaSuccess;
@@ -32,8 +36,18 @@ struct DevBuf {
         if (p && owned) cudaFree(p);
         p = nullptr; cap = 0;
     }
-    template <class T> T *as() { return (T *)p; }
+    template <class T> T *as() const { return (T *)p; }
 };
+
+// device state of each module, defined (and created, see tb2_state) in its own file
+struct BatchHolder;      // resident batch (pipeline.cu)
+struct BatchBuffers;     // arrays of one batch view: the single-read mirrors' own set (pipeline.cu)
+struct LaunchScratch;    // per-launch scratch of tb2_launch_align / tb2_launch_resolve (kernels.h)
+struct DpMirrorState;    // dp_kernels.cu
+struct LlrState;         // llr.cu
+struct RegionState;      // region_stats.cu
+struct GroupState;       // group_stats.cu
+struct DebugState;       // debug.cu
 
 struct tb2_ctx {
     int device = 0;
@@ -45,12 +59,16 @@ struct tb2_ctx {
     std::string err;
     int64_t launches = 0;
     double last_ms_total = 0, last_ms_dp = 0, last_dp_launches = 0, last_dp_reads = 0;
-    std::shared_ptr<void> batch;   // BatchHolder (pipeline.cu)
-    std::shared_ptr<void> region;  // RegionState (region_stats.cu)
-    long long resident_llr_sites = 0;   // tb2_batch_alt_llr: sites / reads of the resident LLRs
-    int resident_llr_reads = 0;
+    std::shared_ptr<BatchHolder> batch;
+    std::shared_ptr<BatchBuffers> one_read;
+    std::shared_ptr<LaunchScratch> launch_scratch;
+    std::shared_ptr<DpMirrorState> dp;
+    std::shared_ptr<LlrState> llr;
+    std::shared_ptr<RegionState> region;
+    std::shared_ptr<GroupState> group;
+    std::shared_ptr<DebugState> debug;
     // tb2_resquiggle_batch pipelines large batches over two lanes (child contexts with
-    // their own stream and pools): H2D of chunk k+1 overlaps the kernels of chunk k
+    // their own stream and buffers): H2D of chunk k+1 overlaps the kernels of chunk k
     std::vector<tb2_ctx *> lanes;
     bool async_mode = false;       // upload / download do not synchronise
     int read_index_base = 0;       // first read of the chunk within the caller's batch
@@ -58,10 +76,6 @@ struct tb2_ctx {
     // model tables
     DevBuf model_means, model_sds, alt_means;
     int kmer_width = 0, central_pos = 0, alt_kmer_width = 0;
-    // generic scratch pool (named slots), grow-only
-    // slots: 0-11 mirror calls, 12-49 batch arrays (pipeline.cu), 50-69 llr.cu,
-    // 70-79 per-warp scratch pools, 80-109 region_stats.cu, 110-124 group_stats.cu
-    std::vector<DevBuf> pool = std::vector<DevBuf>(128);
     // pinned host staging for small results
     void *pinned = nullptr;
     size_t pinned_cap = 0;
@@ -85,6 +99,14 @@ struct tb2_ctx {
         (ctx)->launches++;                                                             \
         TB2_CUDA_TRY(ctx, cudaGetLastError());                                         \
     } while (0)
+
+// a module's state on the context, created on first use.  Called where T is complete: the
+// shared_ptr keeps T's deleter, so tb2_ctx_destroy frees it without knowing the type.
+template <class T> T &tb2_state(std::shared_ptr<T> &state)
+{
+    if (!state) state = std::make_shared<T>();
+    return *state;
+}
 
 static inline int tb2_use(tb2_ctx *ctx)
 {

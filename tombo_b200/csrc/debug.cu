@@ -55,20 +55,23 @@ __global__ void k_div_check(unsigned long long seed, int per_thread, unsigned lo
 }
 }  // namespace
 
+// per-call scratch of tb2_debug_div_check: the mismatch count, then the first example
+struct DebugState { DevBuf out; };
+
 extern "C" int tb2_debug_div_check(tb2_ctx *ctx, uint64_t seed, int blocks, int per_thread,
                                    uint64_t *mismatches, double *example4)
 {
     int rc = tb2_use(ctx);
     if (rc) return rc;
     if (!mismatches || !example4 || blocks < 1 || per_thread < 1) return TB2_ERR_INVALID_ARG;
-    TB2_CUDA_TRY(ctx, ctx->pool[0].reserve(64));
-    TB2_CUDA_TRY(ctx, cudaMemsetAsync(ctx->pool[0].p, 0, 64, ctx->stream));
-    k_div_check<<<blocks, 256, 0, ctx->stream>>>(seed, per_thread,
-                                                 ctx->pool[0].as<unsigned long long>(),
-                                                 ctx->pool[0].as<double>() + 1);
+    DevBuf &out = tb2_state(ctx->debug).out;
+    TB2_CUDA_TRY(ctx, out.reserve(64));
+    TB2_CUDA_TRY(ctx, cudaMemsetAsync(out.p, 0, 64, ctx->stream));
+    k_div_check<<<blocks, 256, 0, ctx->stream>>>(seed, per_thread, out.as<unsigned long long>(),
+                                                 out.as<double>() + 1);
     TB2_CHECK_LAUNCH(ctx);
     unsigned long long h[5];
-    TB2_CUDA_TRY(ctx, cudaMemcpyAsync(h, ctx->pool[0].p, 40, cudaMemcpyDeviceToHost, ctx->stream));
+    TB2_CUDA_TRY(ctx, cudaMemcpyAsync(h, out.p, 40, cudaMemcpyDeviceToHost, ctx->stream));
     TB2_CUDA_TRY(ctx, cudaStreamSynchronize(ctx->stream));
     *mismatches = h[0];
     memcpy(example4, &h[1], 32);

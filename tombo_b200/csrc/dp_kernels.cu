@@ -30,11 +30,11 @@ int tb2_launch_align(tb2_ctx *ctx, const AlignBatch &b, const AlignLaunchCfg &cf
     const int max_useful = (b.n_reads + ALIGN_WARPS - 1) / ALIGN_WARPS;
     if (grid > max_useful) grid = std::max(1, max_useful);
     const size_t slots = (size_t)grid * ALIGN_WARPS;
-    enum { SLOT_TB = 70, SLOT_GROW = 71, SLOT_CNT = 72 };
-    TB2_CUDA_TRY(ctx, ctx->pool[SLOT_TB].reserve(slots * cfg.tb_words * sizeof(uint32_t)));
-    TB2_CUDA_TRY(ctx, ctx->pool[SLOT_GROW].reserve(slots * 2 * (size_t)cfg.grow_cells * sizeof(double) + 8));
-    TB2_CUDA_TRY(ctx, ctx->pool[SLOT_CNT].reserve(sizeof(int)));
-    TB2_CUDA_TRY(ctx, cudaMemsetAsync(ctx->pool[SLOT_CNT].p, 0, sizeof(int), ctx->stream));
+    LaunchScratch &ls = tb2_state(ctx->launch_scratch);
+    TB2_CUDA_TRY(ctx, ls.tb.reserve(slots * cfg.tb_words * sizeof(uint32_t)));
+    TB2_CUDA_TRY(ctx, ls.grow.reserve(slots * 2 * (size_t)cfg.grow_cells * sizeof(double) + 8));
+    TB2_CUDA_TRY(ctx, ls.align_cnt.reserve(sizeof(int)));
+    TB2_CUDA_TRY(ctx, cudaMemsetAsync(ls.align_cnt.p, 0, sizeof(int), ctx->stream));
     auto kern = cfg.klass == 1 ? k_align<1> : (cfg.klass == 2 ? k_align<2> : k_align<0>);
     // (a constant, not this launch's size: contexts launch concurrently from several host
     // threads and the attribute is per function, not per context)
@@ -46,8 +46,7 @@ int tb2_launch_align(tb2_ctx *ctx, const AlignBatch &b, const AlignLaunchCfg &cf
         TB2_CUDA_TRY(ctx, cudaFuncSetAttribute(kern, cudaFuncAttributePreferredSharedMemoryCarveout,
                                                (int)cudaSharedmemCarveoutMaxShared));
     kern<<<grid, ALIGN_WARPS * 32, smem, ctx->stream>>>(
-        b, cfg, ctx->pool[SLOT_TB].as<uint32_t>(), ctx->pool[SLOT_GROW].as<double>(),
-        ctx->pool[SLOT_CNT].as<int>());
+        b, cfg, ls.tb.as<uint32_t>(), ls.grow.as<double>(), ls.align_cnt.as<int>());
     TB2_CHECK_LAUNCH(ctx);
     return TB2_OK;
 }
@@ -164,8 +163,12 @@ __global__ void k_traceback_dbg(const long long *tb, const long long *es, int nb
 // C ABI
 // ---------------------------------------------------------------------------
 namespace {
-enum { S_A = 0, S_B, S_C, S_D, S_E, S_F, S_G, S_H, S_I, S_J, S_K, S_L };
+// per-call scratch of the mirror entry points; nothing reads it after a call returns
+enum { S_A = 0, S_B, S_C, S_D, S_E, S_F, S_G, S_H, S_I, S_J, S_COUNT };
+}  // namespace
+struct DpMirrorState { DevBuf buf[S_COUNT]; };
 
+namespace {
 struct DbgGeom { int smem_cells, grow_cells; size_t smem_bytes; };
 DbgGeom dbg_geom(long long W)
 {
@@ -191,7 +194,7 @@ extern "C" int tb2_banded_forward_pass(tb2_ctx *ctx, const double *z, const int6
         return TB2_ERR_INVALID_ARG;
     if (tb2_row_cells(bw) / 32 > TB2_MAX_WPL * 16) return TB2_ERR_CAPACITY;
     const size_t nz = (size_t)n_bases * bw, nf = (size_t)(n_bases + 1) * bw;
-    auto &P = ctx->pool;
+    auto &P = tb2_state(ctx->dp).buf;
     TB2_CUDA_TRY(ctx, P[S_A].reserve(nz * 8));
     TB2_CUDA_TRY(ctx, P[S_B].reserve(n_bases * 8));
     TB2_CUDA_TRY(ctx, P[S_C].reserve(nf * 8));
@@ -229,7 +232,7 @@ extern "C" int tb2_banded_traceback(tb2_ctx *ctx, const int64_t *tb, const int64
     if (rc) return rc;
     if (!tb || !event_starts || !seq_poss_out || n_bases < 1 || bw < 1) return TB2_ERR_INVALID_ARG;
     const size_t nf = (size_t)(n_bases + 1) * bw;
-    auto &P = ctx->pool;
+    auto &P = tb2_state(ctx->dp).buf;
     TB2_CUDA_TRY(ctx, P[S_A].reserve(nf * 8));
     TB2_CUDA_TRY(ctx, P[S_B].reserve(n_bases * 8));
     TB2_CUDA_TRY(ctx, P[S_C].reserve((n_bases + 1) * 8));
@@ -264,7 +267,7 @@ extern "C" int tb2_adaptive_banded_forward_pass(
         return TB2_ERR_INVALID_ARG;
     if (tb2_row_cells(bw) / 32 > TB2_MAX_WPL * 16) return TB2_ERR_CAPACITY;
     const size_t nf = (size_t)(n_bases + 1) * bw;
-    auto &P = ctx->pool;
+    auto &P = tb2_state(ctx->dp).buf;
     TB2_CUDA_TRY(ctx, P[S_A].reserve(nf * 8));
     TB2_CUDA_TRY(ctx, P[S_B].reserve(nf * 8));
     TB2_CUDA_TRY(ctx, P[S_C].reserve(n_bases * 8));
@@ -335,7 +338,7 @@ extern "C" int tb2_find_adaptive_base_assignment(
     if (!valid_cpts || !event_means || !params || !ref_means || !ref_sds || !segs_out ||
         !read_start_rel_to_raw || n_cpts < 2 || n_bases < 1)
         return TB2_ERR_INVALID_ARG;
-    auto &P = ctx->pool;
+    auto &P = tb2_state(ctx->dp).buf;
     cudaStream_t s = ctx->stream;
     const long long nb = n_bases, n_em = n_cpts - 1;
     std::vector<int> cp32((size_t)n_cpts);
@@ -399,21 +402,6 @@ extern "C" int tb2_find_adaptive_base_assignment(
     return TB2_OK;
 }
 
-// debug aid for parity tests: band starts and event traceback of the last
-// tb2_find_adaptive_base_assignment call on this ctx (n_bases entries / n_bases+1)
-extern "C" int tb2_debug_last_assignment(tb2_ctx *ctx, int64_t n_bases, int64_t *starts_out,
-                                         int64_t *read_tb_out)
-{
-    int rc = tb2_use(ctx);
-    if (rc) return rc;
-    if (n_bases < 1 || !starts_out || !read_tb_out) return TB2_ERR_INVALID_ARG;
-    std::vector<int> h((size_t)(n_bases + 1) * 2);
-    TB2_CUDA_TRY(ctx, cudaMemcpy(h.data(), ctx->pool[S_F].p, h.size() * 4, cudaMemcpyDeviceToHost));
-    for (int64_t i = 0; i < n_bases; ++i) starts_out[i] = h[i];
-    for (int64_t i = 0; i <= n_bases; ++i) read_tb_out[i] = h[(n_bases + 1) + i];
-    return TB2_OK;
-}
-
 // ---------------------------------------------------------------------------
 // single-read mirrors of find_static_base_assignment (resquiggle.py:547-600) and
 // find_seq_start_in_events (resquiggle.py:685-752)
@@ -453,7 +441,7 @@ static int run_single(tb2_ctx *ctx, int mode, const double *em, int64_t n_em, co
     int rc = tb2_use(ctx);
     if (rc) return rc;
     if (!em || !rm || !rs || !p || n_em < 1 || nb < 1) return TB2_ERR_INVALID_ARG;
-    auto &P = ctx->pool;
+    auto &P = tb2_state(ctx->dp).buf;
     cudaStream_t s = ctx->stream;
     const long long W = mode == 0 ? std::max<long long>(1, n_em - std::min<long long>(nb, n_em) / 4)
                                   : num_events;

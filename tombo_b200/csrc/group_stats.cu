@@ -25,8 +25,14 @@
 #include <cmath>
 
 namespace {
-enum { G_LV_S = 110, G_OFF_S, G_ST_S, G_LV_C, G_OFF_C, G_ST_C, G_INT, G_IDX, G_VAL, G_RD, G_SQ,
-       G_RES, G_PRI, G_REF, G_HDR };
+// per-call scratch of tb2_group_reg_stats / tb2_reads_ref_levels; nothing reads it after a
+// call returns
+enum { G_LV_S = 0, G_OFF_S, G_ST_S, G_LV_C, G_OFF_C, G_ST_C, G_INT, G_IDX, G_VAL, G_RD, G_SQ,
+       G_RES, G_PRI, G_REF, G_HDR, G_COUNT };
+}  // namespace
+struct GroupState { DevBuf scratch[G_COUNT]; };
+
+namespace {
 
 constexpr int BT = 256;            // threads of the per-position kernels
 constexpr int G_SH = 5632;         // doubles of shared memory per position (group tests)
@@ -376,7 +382,7 @@ int check_sample(int64_t n, const double *lv, const int64_t *off, const int64_t 
 int upload_sample(tb2_ctx *ctx, int slot, int64_t n, const double *lv, const int64_t *off,
                   const int64_t *st, Sample &s)
 {
-    auto &P = ctx->pool;
+    auto &P = tb2_state(ctx->group).scratch;
     cudaStream_t q = ctx->stream;
     s.n = (int)n;
     s.total = n ? off[n] : 0;
@@ -396,7 +402,7 @@ int upload_sample(tb2_ctx *ctx, int slot, int64_t n, const double *lv, const int
 int gather(tb2_ctx *ctx, long long reg_start, long long reg_len, const Sample &a, const Sample *b,
            int min_reads, int min_run, bool want_reads, long long hdr[4])
 {
-    auto &P = ctx->pool;
+    auto &P = tb2_state(ctx->group).scratch;
     cudaStream_t q = ctx->stream;
     const long long n = reg_len;
     TB2_CUDA_TRY(ctx, P[G_INT].reserve((size_t)n * 5 * 4));
@@ -461,7 +467,7 @@ extern "C" int tb2_group_reg_stats(tb2_ctx *ctx, int64_t reg_start, int64_t reg_
         return TB2_ERR_INVALID_ARG;
     if ((rc = check_sample(n_samp, samp_levels, samp_off, samp_start))) return rc;
     if ((rc = check_sample(n_ctrl, ctrl_levels, ctrl_off, ctrl_start))) return rc;
-    auto &P = ctx->pool;
+    auto &P = tb2_state(ctx->group).scratch;
     cudaStream_t q = ctx->stream;
     Sample a, b;
     if ((rc = upload_sample(ctx, G_LV_S, n_samp, samp_levels, samp_off, samp_start, a))) return rc;
@@ -521,7 +527,7 @@ extern "C" int tb2_reads_ref_levels(tb2_ctx *ctx, int64_t reg_start, int64_t reg
         !means_out || !sds_out || !cov_out || (!prior_means != !prior_sds))
         return TB2_ERR_INVALID_ARG;
     if ((rc = check_sample(n_reads, levels, off, start))) return rc;
-    auto &P = ctx->pool;
+    auto &P = tb2_state(ctx->group).scratch;
     cudaStream_t q = ctx->stream;
     Sample a;
     if ((rc = upload_sample(ctx, G_LV_S, n_reads, levels, off, start, a))) return rc;

@@ -44,6 +44,16 @@ struct AlignLaunchCfg {
 // launches the persistent warp-per-read kernel on ctx->stream
 int tb2_launch_align(tb2_ctx *ctx, const AlignBatch &b, const AlignLaunchCfg &cfg);
 
+#ifndef TB2_EMUL
+// per-warp scratch of k_align (tb2_launch_align) and k_resolve (tb2_launch_resolve).  It holds
+// nothing between launches, and launches on one context are stream-ordered, so the resident
+// batch and the single-read mirrors share it.
+struct LaunchScratch {
+    DevBuf tb, grow, align_cnt;      // k_align: packed moves, global rows, work counter
+    DevBuf raw_dp, resolve_cnt, raw_big;   // k_resolve: per-warp slabs, counters, overflow arena
+};
+#endif
+
 // chunk width of the register engine for the adaptive band (dp_row2.cuh), 0 = band too wide
 #if defined(__CUDACC__) || defined(TB2_EMUL)
 __host__ __device__

@@ -7,8 +7,21 @@
 #include <vector>
 
 namespace {
-enum { L_MEAN = 50, L_MOFF, L_SEQ, L_SOFF, L_START, L_CNT, L_SITEOFF, L_LLR, L_POS, L_A, L_B, L_C, L_D };
+// per-call scratch of the entry points below; nothing reads it after a call returns
+enum { L_MEAN = 0, L_MOFF, L_SEQ, L_SOFF, L_START, L_CNT, L_SITEOFF, L_LLR, L_POS, L_A, L_B, L_C, L_D,
+       L_COUNT };
+}  // namespace
 
+struct LlrState {
+    DevBuf scratch[L_COUNT];
+    // resident LLRs of the last tb2_batch_alt_llr, for tb2_batch_llr_download and
+    // tb2_region_stats_add_batch_llr
+    DevBuf site_off, llr, pos;
+    long long sites = 0;
+    int reads = 0;
+};
+
+namespace {
 struct LlrArgs {
     int n_reads, K, cpos, alt_code, use_std;
     double sf, hf, hp;
@@ -146,7 +159,7 @@ extern "C" int tb2_alt_model_llr_batch(tb2_ctx *ctx, int64_t n_reads, const doub
         const long long nb = mean_off[r + 1] - mean_off[r];
         if (nb < 0 || seq_off[r + 1] - seq_off[r] != nb + (ctx->kmer_width - 1)) return TB2_ERR_INVALID_ARG;
     }
-    auto &P = ctx->pool;
+    auto &P = tb2_state(ctx->llr).scratch;
     cudaStream_t s = ctx->stream;
     const size_t tm = (size_t)mean_off[n], ts = (size_t)seq_off[n];
     TB2_CUDA_TRY(ctx, P[L_MEAN].reserve(tm * 8 + 8));
@@ -226,7 +239,6 @@ __global__ void __launch_bounds__(1024) k_scan_sites(const int *cnt, long long *
         __syncthreads();
     }
 }
-enum { L_RSTART = 63, L_RCNT, L_RSITEOFF, L_RLLR, L_RPOS, L_RTOTAL };
 }  // namespace
 
 extern "C" int tb2_batch_alt_llr(tb2_ctx *ctx, const int64_t *read_start, int alt_base_code,
@@ -243,37 +255,38 @@ extern "C" int tb2_batch_alt_llr(tb2_ctx *ctx, const int64_t *read_start, int al
     BatchResultView v;
     if ((rc = tb2_batch_result_view(ctx, &v))) return rc;
     const int n = v.n_reads;
-    auto &P = ctx->pool;
+    LlrState &L = tb2_state(ctx->llr);
+    auto &P = L.scratch;
     cudaStream_t s = ctx->stream;
-    TB2_CUDA_TRY(ctx, P[L_RSTART].reserve((size_t)n * 8));
-    TB2_CUDA_TRY(ctx, P[L_RCNT].reserve((size_t)n * 4));
-    TB2_CUDA_TRY(ctx, P[L_RSITEOFF].reserve((size_t)(n + 1) * 8));
+    TB2_CUDA_TRY(ctx, P[L_START].reserve((size_t)n * 8));
+    TB2_CUDA_TRY(ctx, P[L_CNT].reserve((size_t)n * 4));
+    TB2_CUDA_TRY(ctx, L.site_off.reserve((size_t)(n + 1) * 8));
     // every site is a base: the batch's base count bounds the site count (no size round trip)
-    TB2_CUDA_TRY(ctx, P[L_RLLR].reserve((size_t)v.total_bases * 8 + 8));
-    TB2_CUDA_TRY(ctx, P[L_RPOS].reserve((size_t)v.total_bases * 8 + 8));
-    TB2_CUDA_TRY(ctx, cudaMemcpyAsync(P[L_RSTART].p, read_start, (size_t)n * 8, cudaMemcpyHostToDevice, s));
+    TB2_CUDA_TRY(ctx, L.llr.reserve((size_t)v.total_bases * 8 + 8));
+    TB2_CUDA_TRY(ctx, L.pos.reserve((size_t)v.total_bases * 8 + 8));
+    TB2_CUDA_TRY(ctx, cudaMemcpyAsync(P[L_START].p, read_start, (size_t)n * 8, cudaMemcpyHostToDevice, s));
     LlrArgs a;
     a.n_reads = n; a.K = ctx->kmer_width; a.cpos = ctx->central_pos; a.alt_code = alt_base_code;
     a.use_std = use_standard_llhr ? 1 : 0;
     a.sf = scale_factor; a.hf = height_factor; a.hp = height_power;
     a.norm_mean = v.norm_mean; a.mean_off = v.base_off; a.seq_off = v.seq_off;
-    a.read_start = P[L_RSTART].as<long long>();
+    a.read_start = P[L_START].as<long long>();
     a.seq = v.seq;
     a.kmeans = ctx->model_means.as<double>(); a.ksds = ctx->model_sds.as<double>();
     a.alt = ctx->alt_means.as<double>();
     a.status = v.status; a.status_stride = v.stride;
-    k_llr<false><<<n, 256, 0, s>>>(a, P[L_RCNT].as<int>(), nullptr, nullptr, nullptr);
+    k_llr<false><<<n, 256, 0, s>>>(a, P[L_CNT].as<int>(), nullptr, nullptr, nullptr);
     TB2_CHECK_LAUNCH(ctx);
-    k_scan_sites<<<1, 1024, 0, s>>>(P[L_RCNT].as<int>(), P[L_RSITEOFF].as<long long>(), n);
+    k_scan_sites<<<1, 1024, 0, s>>>(P[L_CNT].as<int>(), L.site_off.as<long long>(), n);
     TB2_CHECK_LAUNCH(ctx);
-    k_llr<true><<<n, 256, 0, s>>>(a, nullptr, P[L_RSITEOFF].as<long long>(), P[L_RLLR].as<double>(),
-                                  P[L_RPOS].as<long long>());
+    k_llr<true><<<n, 256, 0, s>>>(a, nullptr, L.site_off.as<long long>(), L.llr.as<double>(),
+                                  L.pos.as<long long>());
     TB2_CHECK_LAUNCH(ctx);
     long long total = 0;
-    TB2_CUDA_TRY(ctx, cudaMemcpyAsync(&total, P[L_RSITEOFF].as<long long>() + n, 8, cudaMemcpyDeviceToHost, s));
+    TB2_CUDA_TRY(ctx, cudaMemcpyAsync(&total, L.site_off.as<long long>() + n, 8, cudaMemcpyDeviceToHost, s));
     TB2_CUDA_TRY(ctx, cudaStreamSynchronize(s));
-    ctx->resident_llr_sites = total;
-    ctx->resident_llr_reads = n;
+    L.sites = total;
+    L.reads = n;
     if (n_sites_total) *n_sites_total = total;
     return TB2_OK;
 }
@@ -282,15 +295,15 @@ extern "C" int tb2_batch_llr_download(tb2_ctx *ctx, double *llr_out, int64_t *po
 {
     int rc = tb2_use(ctx);
     if (rc) return rc;
-    if (ctx->resident_llr_reads <= 0 || !site_off) return TB2_ERR_INVALID_ARG;
-    auto &P = ctx->pool;
+    const LlrState &L = tb2_state(ctx->llr);
+    if (L.reads <= 0 || !site_off) return TB2_ERR_INVALID_ARG;
     cudaStream_t s = ctx->stream;
-    const size_t t = (size_t)ctx->resident_llr_sites;
+    const size_t t = (size_t)L.sites;
     if (t && (!llr_out || !pos_out)) return TB2_ERR_INVALID_ARG;
-    TB2_CUDA_TRY(ctx, cudaMemcpyAsync(site_off, P[L_RSITEOFF].p, (size_t)(ctx->resident_llr_reads + 1) * 8, cudaMemcpyDeviceToHost, s));
+    TB2_CUDA_TRY(ctx, cudaMemcpyAsync(site_off, L.site_off.p, (size_t)(L.reads + 1) * 8, cudaMemcpyDeviceToHost, s));
     if (t) {
-        TB2_CUDA_TRY(ctx, cudaMemcpyAsync(llr_out, P[L_RLLR].p, t * 8, cudaMemcpyDeviceToHost, s));
-        TB2_CUDA_TRY(ctx, cudaMemcpyAsync(pos_out, P[L_RPOS].p, t * 8, cudaMemcpyDeviceToHost, s));
+        TB2_CUDA_TRY(ctx, cudaMemcpyAsync(llr_out, L.llr.p, t * 8, cudaMemcpyDeviceToHost, s));
+        TB2_CUDA_TRY(ctx, cudaMemcpyAsync(pos_out, L.pos.p, t * 8, cudaMemcpyDeviceToHost, s));
     }
     TB2_CUDA_TRY(ctx, cudaStreamSynchronize(s));
     return TB2_OK;
@@ -302,10 +315,10 @@ extern "C" int tb2_region_stats_add_batch_llr(tb2_ctx *ctx, double single_read_t
 {
     int rc = tb2_use(ctx);
     if (rc) return rc;
-    if (ctx->resident_llr_reads <= 0 || isnan(single_read_thresh)) return TB2_ERR_INVALID_ARG;
-    return tb2_region_accumulate_dev(ctx, ctx->resident_llr_sites, ctx->pool[L_RLLR].as<double>(),
-                                     ctx->pool[L_RPOS].as<long long>(), single_read_thresh,
-                                     lower_thresh, stat_type);
+    LlrState &L = tb2_state(ctx->llr);
+    if (L.reads <= 0 || isnan(single_read_thresh)) return TB2_ERR_INVALID_ARG;
+    return tb2_region_accumulate_dev(ctx, L.sites, L.llr.as<double>(), L.pos.as<long long>(),
+                                     single_read_thresh, lower_thresh, stat_type);
 }
 
 extern "C" int tb2_new_mean_stds(tb2_ctx *ctx, const double *sig, int64_t n_sig,
@@ -317,7 +330,7 @@ extern "C" int tb2_new_mean_stds(tb2_ctx *ctx, const double *sig, int64_t n_sig,
     if (!sig || !segs || !means_out || !sds_out || n_sig < 1 || n_segs < 1) return TB2_ERR_INVALID_ARG;
     for (int64_t i = 0; i <= n_segs; ++i)
         if (segs[i] < 0 || segs[i] > n_sig) return TB2_ERR_INVALID_ARG;
-    auto &P = ctx->pool;
+    auto &P = tb2_state(ctx->llr).scratch;
     cudaStream_t s = ctx->stream;
     TB2_CUDA_TRY(ctx, P[L_A].reserve((size_t)n_sig * 8));
     TB2_CUDA_TRY(ctx, P[L_B].reserve((size_t)(n_segs + 1) * 8));
@@ -397,7 +410,7 @@ extern "C" int tb2_calc_llh_ratio_windows(tb2_ctx *ctx, int mode, int64_t n_site
         return TB2_ERR_INVALID_ARG;
     if (n_sites == 0) return TB2_OK;
     if (!means || !ref_means || !alt_means || !llr_out) return TB2_ERR_INVALID_ARG;
-    auto &P = ctx->pool;
+    auto &P = tb2_state(ctx->llr).scratch;
     cudaStream_t s = ctx->stream;
     const size_t nk = (size_t)n_sites * kmer_width * 8, nv = (size_t)n_sites * 8;
     TB2_CUDA_TRY(ctx, P[L_MEAN].reserve(nk));

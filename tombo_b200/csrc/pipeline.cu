@@ -19,15 +19,16 @@
 int tb2_launch_start_attempt(tb2_ctx *ctx, const BatchView &b, int attempt);
 int tb2_launch_end_call(tb2_ctx *ctx, const BatchView &b, int max_iters);
 
-namespace {
-
-// pool slots of the batch arrays (mirror DP calls use slots 0..11 transiently)
-enum {
-    B_RAWOFF = 12, B_SEQOFF, B_BASEOFF, B_EVOFF, B_SEQ, B_RAWIN, B_RAWF, B_NORM, B_CS, B_SCORES,
-    B_CSTATE, B_CPTS, B_EM, B_RM, B_RS, B_BM, B_TMPB, B_STARTS, B_READTB, B_SEGSDP, B_SEGS,
-    B_STALLS, B_STATE, B_DBG, B_COUNTERS, B_OUT_SEGS, B_OUT_NORMMEAN, B_OUT_NORMSIG, B_OUT_SMALL,
-    B_SVIN, B_NSTALL, B_ORDER
+// device arrays behind one BatchView (build_view).  The resident batch owns one set; the
+// single-read mirrors build their views in a second set, so they never touch a resident batch.
+struct BatchBuffers {
+    DevBuf raw_off, seq_off, base_off, ev_off, seq, rawf, norm, cs, scores, cstate, cpts, em, rm, rs,
+        bm, tmp_b, starts, read_tb, segs_dp, segs, stalls, state, order;
+    DevBuf dbg;        // k_align: 3 ints per read
+    DevBuf counters;   // tb2_launch_count_active
 };
+
+namespace {
 
 // optional caller-provided per-read inputs of resquiggle_read: map_res.scale_values
 // and map_res.stall_ints (resquiggle.py:1079-1084, 1101-1103)
@@ -53,8 +54,9 @@ long long num_events_of(long long n_raw, long long nb, const tb2_params &p, doub
     return a > c ? a : c;
 }
 
-int build_view(tb2_ctx *ctx, int n, const int64_t *raw_off, const int64_t *seq_off, int K,
-               const tb2_params &p, double ratio, int is_rna, HostBatch &hb, BatchView &v)
+// fills B for n reads and points v into it
+int build_view(tb2_ctx *ctx, BatchBuffers &B, int n, const int64_t *raw_off, const int64_t *seq_off,
+               int K, const tb2_params &p, double ratio, int is_rna, HostBatch &hb, BatchView &v)
 {
     hb.n = n;
     long long max_raw_pre = 0;
@@ -77,40 +79,39 @@ int build_view(tb2_ctx *ctx, int n, const int64_t *raw_off, const int64_t *seq_o
     hb.total_b = hb.base_off[n];
     hb.total_e = hb.ev_off[n];
     if (raw_off[0] != 0 || seq_off[0] != 0) return TB2_ERR_INVALID_ARG;
-    auto &P = ctx->pool;
     const size_t S = (size_t)hb.total_s, Bn = (size_t)hb.total_b, E = (size_t)hb.total_e;
     // a stall needs > 200 consecutive observations (MEAN_STALL_PARAMS), so a read of S
     // samples holds at most S / 200 + 1 intervals: size the slots from the longest read
     const int stall_cap = (int)std::max<long long>(8, max_raw_pre / 200 + 4);
-    TB2_CUDA_TRY(ctx, P[B_RAWOFF].reserve((n + 1) * 8));
-    TB2_CUDA_TRY(ctx, P[B_SEQOFF].reserve((n + 1) * 8));
-    TB2_CUDA_TRY(ctx, P[B_BASEOFF].reserve((n + 1) * 8));
-    TB2_CUDA_TRY(ctx, P[B_EVOFF].reserve((n + 1) * 8));
-    TB2_CUDA_TRY(ctx, P[B_SEQ].reserve((size_t)hb.total_seq + 8));
-    TB2_CUDA_TRY(ctx, P[B_RAWF].reserve(S * 8 + 8));
-    TB2_CUDA_TRY(ctx, P[B_NORM].reserve(S * 8 + 8));
-    TB2_CUDA_TRY(ctx, P[B_CS].reserve((S + n) * 8 + 8));
-    TB2_CUDA_TRY(ctx, P[B_SCORES].reserve(S * 8 + 8));
-    TB2_CUDA_TRY(ctx, P[B_CSTATE].reserve(2 * S + 128 * (size_t)n + 16));
-    TB2_CUDA_TRY(ctx, P[B_CPTS].reserve(E * 4 + 8));
-    TB2_CUDA_TRY(ctx, P[B_EM].reserve(E * 8 + 8));
-    TB2_CUDA_TRY(ctx, P[B_RM].reserve(Bn * 8 + 8));
-    TB2_CUDA_TRY(ctx, P[B_RS].reserve(Bn * 8 + 8));
-    TB2_CUDA_TRY(ctx, P[B_BM].reserve(Bn * 8 + 8));
-    TB2_CUDA_TRY(ctx, P[B_TMPB].reserve((Bn + n) * 8 + 8));
-    TB2_CUDA_TRY(ctx, P[B_STARTS].reserve(Bn * 4 + 8));
-    TB2_CUDA_TRY(ctx, P[B_READTB].reserve((Bn + n) * 4 + 8));
-    TB2_CUDA_TRY(ctx, P[B_SEGSDP].reserve((Bn + n) * 4 + 8));
-    TB2_CUDA_TRY(ctx, P[B_SEGS].reserve((Bn + n) * 4 + 8));
-    TB2_CUDA_TRY(ctx, P[B_STALLS].reserve(is_rna ? (size_t)n * 2 * stall_cap * 4 + 8 : 8));
-    TB2_CUDA_TRY(ctx, P[B_STATE].reserve((size_t)n * sizeof(ReadState)));
-    TB2_CUDA_TRY(ctx, P[B_DBG].reserve((size_t)n * 3 * 4));
-    TB2_CUDA_TRY(ctx, P[B_COUNTERS].reserve(64));
+    TB2_CUDA_TRY(ctx, B.raw_off.reserve((n + 1) * 8));
+    TB2_CUDA_TRY(ctx, B.seq_off.reserve((n + 1) * 8));
+    TB2_CUDA_TRY(ctx, B.base_off.reserve((n + 1) * 8));
+    TB2_CUDA_TRY(ctx, B.ev_off.reserve((n + 1) * 8));
+    TB2_CUDA_TRY(ctx, B.seq.reserve((size_t)hb.total_seq + 8));
+    TB2_CUDA_TRY(ctx, B.rawf.reserve(S * 8 + 8));
+    TB2_CUDA_TRY(ctx, B.norm.reserve(S * 8 + 8));
+    TB2_CUDA_TRY(ctx, B.cs.reserve((S + n) * 8 + 8));
+    TB2_CUDA_TRY(ctx, B.scores.reserve(S * 8 + 8));
+    TB2_CUDA_TRY(ctx, B.cstate.reserve(2 * S + 128 * (size_t)n + 16));
+    TB2_CUDA_TRY(ctx, B.cpts.reserve(E * 4 + 8));
+    TB2_CUDA_TRY(ctx, B.em.reserve(E * 8 + 8));
+    TB2_CUDA_TRY(ctx, B.rm.reserve(Bn * 8 + 8));
+    TB2_CUDA_TRY(ctx, B.rs.reserve(Bn * 8 + 8));
+    TB2_CUDA_TRY(ctx, B.bm.reserve(Bn * 8 + 8));
+    TB2_CUDA_TRY(ctx, B.tmp_b.reserve((Bn + n) * 8 + 8));
+    TB2_CUDA_TRY(ctx, B.starts.reserve(Bn * 4 + 8));
+    TB2_CUDA_TRY(ctx, B.read_tb.reserve((Bn + n) * 4 + 8));
+    TB2_CUDA_TRY(ctx, B.segs_dp.reserve((Bn + n) * 4 + 8));
+    TB2_CUDA_TRY(ctx, B.segs.reserve((Bn + n) * 4 + 8));
+    TB2_CUDA_TRY(ctx, B.stalls.reserve(is_rna ? (size_t)n * 2 * stall_cap * 4 + 8 : 8));
+    TB2_CUDA_TRY(ctx, B.state.reserve((size_t)n * sizeof(ReadState)));
+    TB2_CUDA_TRY(ctx, B.dbg.reserve((size_t)n * 3 * 4));
+    TB2_CUDA_TRY(ctx, B.counters.reserve(64));
     cudaStream_t s = ctx->stream;
-    TB2_CUDA_TRY(ctx, cudaMemcpyAsync(P[B_RAWOFF].p, raw_off, (n + 1) * 8, cudaMemcpyHostToDevice, s));
-    TB2_CUDA_TRY(ctx, cudaMemcpyAsync(P[B_SEQOFF].p, seq_off, (n + 1) * 8, cudaMemcpyHostToDevice, s));
-    TB2_CUDA_TRY(ctx, cudaMemcpyAsync(P[B_BASEOFF].p, hb.base_off.data(), (n + 1) * 8, cudaMemcpyHostToDevice, s));
-    TB2_CUDA_TRY(ctx, cudaMemcpyAsync(P[B_EVOFF].p, hb.ev_off.data(), (n + 1) * 8, cudaMemcpyHostToDevice, s));
+    TB2_CUDA_TRY(ctx, cudaMemcpyAsync(B.raw_off.p, raw_off, (n + 1) * 8, cudaMemcpyHostToDevice, s));
+    TB2_CUDA_TRY(ctx, cudaMemcpyAsync(B.seq_off.p, seq_off, (n + 1) * 8, cudaMemcpyHostToDevice, s));
+    TB2_CUDA_TRY(ctx, cudaMemcpyAsync(B.base_off.p, hb.base_off.data(), (n + 1) * 8, cudaMemcpyHostToDevice, s));
+    TB2_CUDA_TRY(ctx, cudaMemcpyAsync(B.ev_off.p, hb.ev_off.data(), (n + 1) * 8, cudaMemcpyHostToDevice, s));
     // launch order: longest reads first, so that the persistent DP warps and the
     // CTA-per-read kernels do not end on a straggler (length bucketing of mixed batches)
     v.order = nullptr;
@@ -123,37 +124,37 @@ int build_view(tb2_ctx *ctx, int n, const int64_t *raw_off, const int64_t *seq_o
             std::stable_sort(order.begin(), order.end(), [&](int a, int b) {
                 return raw_off[a + 1] - raw_off[a] > raw_off[b + 1] - raw_off[b];
             });
-            TB2_CUDA_TRY(ctx, P[B_ORDER].reserve((size_t)n * 4));
-            TB2_CUDA_TRY(ctx, cudaMemcpyAsync(P[B_ORDER].p, order.data(), (size_t)n * 4, cudaMemcpyHostToDevice, s));
+            TB2_CUDA_TRY(ctx, B.order.reserve((size_t)n * 4));
+            TB2_CUDA_TRY(ctx, cudaMemcpyAsync(B.order.p, order.data(), (size_t)n * 4, cudaMemcpyHostToDevice, s));
             TB2_CUDA_TRY(ctx, cudaStreamSynchronize(s));   // order is a local
-            v.order = P[B_ORDER].as<int>();
+            v.order = B.order.as<int>();
         }
     }
     v.n_reads = n;
     v.kmer_width = K;
-    v.raw_off = P[B_RAWOFF].as<long long>();
-    v.seq_off = P[B_SEQOFF].as<long long>();
-    v.base_off = P[B_BASEOFF].as<long long>();
-    v.ev_off = P[B_EVOFF].as<long long>();
-    v.seq = P[B_SEQ].as<unsigned char>();
-    v.rawf = P[B_RAWF].as<double>();
-    v.norm = P[B_NORM].as<double>();
-    v.cs = P[B_CS].as<double>();
-    v.scores = P[B_SCORES].as<double>();
-    v.cstate = P[B_CSTATE].as<unsigned char>();
-    v.cpts = P[B_CPTS].as<int>();
-    v.em = P[B_EM].as<double>();
-    v.rm = P[B_RM].as<double>();
-    v.rs = P[B_RS].as<double>();
-    v.bm = P[B_BM].as<double>();
-    v.tmp_b = P[B_TMPB].as<double>();
-    v.starts = P[B_STARTS].as<int>();
-    v.read_tb = P[B_READTB].as<int>();
-    v.segs_dp = P[B_SEGSDP].as<int>();
-    v.segs = P[B_SEGS].as<int>();
-    v.stall_ints = is_rna ? P[B_STALLS].as<int>() : nullptr;
+    v.raw_off = B.raw_off.as<long long>();
+    v.seq_off = B.seq_off.as<long long>();
+    v.base_off = B.base_off.as<long long>();
+    v.ev_off = B.ev_off.as<long long>();
+    v.seq = B.seq.as<unsigned char>();
+    v.rawf = B.rawf.as<double>();
+    v.norm = B.norm.as<double>();
+    v.cs = B.cs.as<double>();
+    v.scores = B.scores.as<double>();
+    v.cstate = B.cstate.as<unsigned char>();
+    v.cpts = B.cpts.as<int>();
+    v.em = B.em.as<double>();
+    v.rm = B.rm.as<double>();
+    v.rs = B.rs.as<double>();
+    v.bm = B.bm.as<double>();
+    v.tmp_b = B.tmp_b.as<double>();
+    v.starts = B.starts.as<int>();
+    v.read_tb = B.read_tb.as<int>();
+    v.segs_dp = B.segs_dp.as<int>();
+    v.segs = B.segs.as<int>();
+    v.stall_ints = is_rna ? B.stalls.as<int>() : nullptr;
     v.stall_cap = stall_cap;
-    v.st = P[B_STATE].as<ReadState>();
+    v.st = B.state.as<ReadState>();
     return TB2_OK;
 }
 
@@ -248,7 +249,8 @@ StagePolicy stage_policy(const tb2_policy &pl)
     return sp;
 }
 
-AlignBatch make_align_batch(tb2_ctx *ctx, const BatchView &v, const tb2_params &p, double thresh)
+AlignBatch make_align_batch(const BatchBuffers &B, const BatchView &v, const tb2_params &p,
+                            double thresh)
 {
     AlignBatch ab;
     ab.n_reads = v.n_reads;
@@ -262,14 +264,15 @@ AlignBatch make_align_batch(tb2_ctx *ctx, const BatchView &v, const tb2_params &
     ab.rsrtr = &v.st[0].rsrtr;
     ab.status = &v.st[0].status;
     ab.active = &v.st[0].active;
-    ab.dbg = ctx->pool[B_DBG].as<int>();
+    ab.dbg = B.dbg.as<int>();
     ab.params = p;
     ab.sig_match_thresh = thresh;
     return ab;
 }
 
 // one resquiggle_read call over the batch (all active reads)
-int run_call(tb2_ctx *ctx, const BatchView &v, const tb2_params &p, const StagePolicy &sp,
+int run_call(tb2_ctx *ctx, const BatchBuffers &B, const BatchView &v, const tb2_params &p,
+             const StagePolicy &sp,
              const AlignLaunchCfg *acfg /* [2]: short, long; tb_words 0 = class empty */,
              int first_call, double *norm_mean_dev,
              double *norm_sig_dev, size_t rawdp_cap)
@@ -290,7 +293,7 @@ int run_call(tb2_ctx *ctx, const BatchView &v, const tb2_params &p, const StageP
     TB2_CUDA_TRY(ctx, cudaEventRecord(ctx->ev2, ctx->stream));
     for (int k = 0; k < 2; ++k)
         if (acfg[k].tb_words > 0 &&
-            (rc = tb2_launch_align(ctx, make_align_batch(ctx, v, p, sp.sig_match_thresh), acfg[k])))
+            (rc = tb2_launch_align(ctx, make_align_batch(B, v, p, sp.sig_match_thresh), acfg[k])))
             return rc;
     TB2_CUDA_TRY(ctx, cudaEventRecord(ctx->ev3, ctx->stream));
     if ((rc = tb2_launch_resolve(ctx, v, p, sp, rawdp_cap))) return rc;
@@ -327,7 +330,6 @@ extern "C" int tb2_set_model(tb2_ctx *ctx, const double *means, const double *sd
 // batched hot path in three stages: upload (H2D), compute (kernels only; results
 // stay on the device), download (D2H).  tb2_resquiggle_batch = all three.
 // ---------------------------------------------------------------------------
-namespace {
 struct BatchHolder {
     HostBatch hb;
     BatchView v;
@@ -335,12 +337,33 @@ struct BatchHolder {
     int raw_dtype = 0;
     bool uploaded = false, computed = false, has_norm_sig = false;
     bool has_sv_in = false, has_stalls_in = false;
+    BatchBuffers buf;                  // behind v
+    DevBuf raw_in, sv_in, n_stall;     // uploaded signal, tb2_batch_set_read_inputs
+    // export staging: segs (int64), norm_mean, norm_signal, and the per-read results (SmallOut)
+    DevBuf out_segs, out_norm_mean, out_norm_sig, out_small;
 };
 
-BatchHolder *holder_of(tb2_ctx *ctx)
+namespace {
+BatchHolder *holder_of(tb2_ctx *ctx) { return &tb2_state(ctx->batch); }
+
+// layout of BatchHolder::out_small: six per-read arrays back to back
+struct SmallOut {
+    long long *rsrtr;
+    tb2_scale_values *sv;
+    double *score;
+    int *status, *n_iters, *flags;
+};
+size_t small_out_bytes(int n) { return (size_t)n * (8 + sizeof(tb2_scale_values) + 8 + 4 + 4 + 4); }
+SmallOut small_out(const DevBuf &b, int n)
 {
-    if (!ctx->batch) ctx->batch = std::shared_ptr<void>(new BatchHolder(), [](void *p) { delete (BatchHolder *)p; });
-    return (BatchHolder *)ctx->batch.get();
+    SmallOut o;
+    o.rsrtr = b.as<long long>();
+    o.sv = (tb2_scale_values *)(o.rsrtr + n);
+    o.score = (double *)(o.sv + n);
+    o.status = (int *)(o.score + n);
+    o.n_iters = o.status + n;
+    o.flags = o.n_iters + n;
+    return o;
 }
 }  // namespace
 
@@ -357,24 +380,23 @@ static int batch_upload_impl(tb2_ctx *ctx, int64_t n_reads, const void *raw, int
     BatchHolder *h = holder_of(ctx);
     h->uploaded = h->computed = false;
     const int n = (int)n_reads;
-    rc = build_view(ctx, n, raw_off, seq_off, ctx->kmer_width, *params,
+    rc = build_view(ctx, h->buf, n, raw_off, seq_off, ctx->kmer_width, *params,
                     policy->min_event_to_seq_ratio, (int)policy->is_rna, h->hb, h->v);
     if (rc) return rc;
     h->raw_off.assign(raw_off, raw_off + n + 1);
     h->raw_dtype = raw_dtype;
-    auto &P = ctx->pool;
     cudaStream_t s = ctx->stream;
     const size_t esz = raw_dtype == 0 ? 8 : 2;
-    TB2_CUDA_TRY(ctx, P[B_RAWIN].reserve((size_t)h->hb.total_s * esz + 8));
+    TB2_CUDA_TRY(ctx, h->raw_in.reserve((size_t)h->hb.total_s * esz + 8));
     // the (small, possibly pageable) sequence copy goes first: a pageable source blocks the
     // host until the copy has run, and behind the big signal copy that would serialise
     // the pipelined path (H2D of chunk k+1 must overlap the kernels of chunk k)
-    TB2_CUDA_TRY(ctx, cudaMemcpyAsync(P[B_SEQ].p, seq, (size_t)h->hb.total_seq, cudaMemcpyHostToDevice, s));
+    TB2_CUDA_TRY(ctx, cudaMemcpyAsync(h->buf.seq.p, seq, (size_t)h->hb.total_seq, cudaMemcpyHostToDevice, s));
     if (getenv("TB2_TRACE")) {
         if (!ctx->ev_h0) { cudaEventCreate(&ctx->ev_h0); cudaEventCreate(&ctx->ev_h1); }
         cudaEventRecord(ctx->ev_h0, s);
     }
-    TB2_CUDA_TRY(ctx, cudaMemcpyAsync(P[B_RAWIN].p, raw, (size_t)h->hb.total_s * esz, cudaMemcpyHostToDevice, s));
+    TB2_CUDA_TRY(ctx, cudaMemcpyAsync(h->raw_in.p, raw, (size_t)h->hb.total_s * esz, cudaMemcpyHostToDevice, s));
     if (ctx->ev_h1) cudaEventRecord(ctx->ev_h1, s);
     if (!ctx->async_mode) TB2_CUDA_TRY(ctx, cudaStreamSynchronize(s));
     h->uploaded = true;
@@ -390,12 +412,11 @@ static int batch_set_read_inputs_impl(tb2_ctx *ctx, const tb2_scale_values *sv_i
     BatchHolder *h = holder_of(ctx);
     if (!h->uploaded) { ctx->err = "tb2_batch_upload has not been called"; return TB2_ERR_INVALID_ARG; }
     const int n = h->hb.n;
-    auto &P = ctx->pool;
     cudaStream_t s = ctx->stream;
     h->has_sv_in = sv_in != nullptr;
     if (sv_in) {
-        TB2_CUDA_TRY(ctx, P[B_SVIN].reserve((size_t)n * sizeof(tb2_scale_values)));
-        TB2_CUDA_TRY(ctx, cudaMemcpyAsync(P[B_SVIN].p, sv_in, (size_t)n * sizeof(tb2_scale_values), cudaMemcpyHostToDevice, s));
+        TB2_CUDA_TRY(ctx, h->sv_in.reserve((size_t)n * sizeof(tb2_scale_values)));
+        TB2_CUDA_TRY(ctx, cudaMemcpyAsync(h->sv_in.p, sv_in, (size_t)n * sizeof(tb2_scale_values), cudaMemcpyHostToDevice, s));
     }
     h->has_stalls_in = stall_off != nullptr;
     if (stall_off) {
@@ -409,11 +430,11 @@ static int batch_set_read_inputs_impl(tb2_ctx *ctx, const tb2_scale_values *sv_i
                 flat[((size_t)r * cap + k) * 2 + 1] = (int)stall_ints[2 * (stall_off[r] + k) + 1];
             }
         }
-        TB2_CUDA_TRY(ctx, P[B_STALLS].reserve(flat.size() * 4 + 8));
-        TB2_CUDA_TRY(ctx, P[B_NSTALL].reserve((size_t)n * 4));
-        TB2_CUDA_TRY(ctx, cudaMemcpyAsync(P[B_STALLS].p, flat.data(), flat.size() * 4, cudaMemcpyHostToDevice, s));
-        TB2_CUDA_TRY(ctx, cudaMemcpyAsync(P[B_NSTALL].p, cnt.data(), (size_t)n * 4, cudaMemcpyHostToDevice, s));
-        h->v.stall_ints = P[B_STALLS].as<int>();
+        TB2_CUDA_TRY(ctx, h->buf.stalls.reserve(flat.size() * 4 + 8));
+        TB2_CUDA_TRY(ctx, h->n_stall.reserve((size_t)n * 4));
+        TB2_CUDA_TRY(ctx, cudaMemcpyAsync(h->buf.stalls.p, flat.data(), flat.size() * 4, cudaMemcpyHostToDevice, s));
+        TB2_CUDA_TRY(ctx, cudaMemcpyAsync(h->n_stall.p, cnt.data(), (size_t)n * 4, cudaMemcpyHostToDevice, s));
+        h->v.stall_ints = h->buf.stalls.as<int>();
         h->v.stall_cap = cap;
     }
     TB2_CUDA_TRY(ctx, cudaStreamSynchronize(s));
@@ -436,7 +457,6 @@ static int batch_compute_impl(tb2_ctx *ctx, const tb2_params *params,
     const HostBatch &hb = h->hb;
     const BatchView &v = h->v;
     const int n = hb.n;
-    auto &P = ctx->pool;
     cudaStream_t s = ctx->stream;
     const bool trace = getenv("TB2_TRACE") != nullptr;
     auto now_ms = [] {
@@ -444,15 +464,15 @@ static int batch_compute_impl(tb2_ctx *ctx, const tb2_params *params,
     };
     const double tc0 = now_ms();
     TB2_CUDA_TRY(ctx, cudaEventRecord(ctx->ev0, s));
-    TB2_CUDA_TRY(ctx, P[B_OUT_NORMMEAN].reserve((size_t)hb.total_b * 8 + 8));
+    TB2_CUDA_TRY(ctx, h->out_norm_mean.reserve((size_t)hb.total_b * 8 + 8));
     double *norm_sig_dev = nullptr;
     if (want_norm_signal) {
-        TB2_CUDA_TRY(ctx, P[B_OUT_NORMSIG].reserve((size_t)hb.total_s * 8 + 8));
-        norm_sig_dev = P[B_OUT_NORMSIG].as<double>();
+        TB2_CUDA_TRY(ctx, h->out_norm_sig.reserve((size_t)hb.total_s * 8 + 8));
+        norm_sig_dev = h->out_norm_sig.as<double>();
     }
     h->has_norm_sig = want_norm_signal != 0;
-    double *norm_mean_dev = P[B_OUT_NORMMEAN].as<double>();
-    if ((rc = tb2_launch_prep(ctx, v, P[B_RAWIN].p, h->raw_dtype, sp.is_rna, hb.total_s, hb.total_b))) return rc;
+    double *norm_mean_dev = h->out_norm_mean.as<double>();
+    if ((rc = tb2_launch_prep(ctx, v, h->raw_in.p, h->raw_dtype, sp.is_rna, hb.total_s, hb.total_b))) return rc;
     if (sp.is_rna && !h->has_stalls_in && (rc = tb2_launch_stalls(ctx, v))) return rc;
     const size_t rawdp_cap = (size_t)1 << 15;
     double ms_dp = 0, dp_reads = 0;
@@ -470,15 +490,15 @@ static int batch_compute_impl(tb2_ctx *ctx, const tb2_params *params,
         if ((rc = tb2_launch_start_attempt(ctx, v, attempt))) return rc;
         if (h->has_sv_in || h->has_stalls_in) {
             k_apply_inputs<<<(n + 255) / 256, 256, 0, s>>>(
-                v, h->has_sv_in ? P[B_SVIN].as<tb2_scale_values>() : nullptr,
-                h->has_stalls_in ? P[B_NSTALL].as<int>() : nullptr);
+                v, h->has_sv_in ? h->sv_in.as<tb2_scale_values>() : nullptr,
+                h->has_stalls_in ? h->n_stall.as<int>() : nullptr);
             TB2_CHECK_LAUNCH(ctx);
         }
         double active_now = attempt == 0 ? n : counters[1];
         for (int it = 0; it < std::max(1, sp.max_scaling_iters); ++it) {
-            if ((rc = run_call(ctx, v, p, sp, acfg, it == 0, norm_mean_dev, norm_sig_dev, rawdp_cap)))
+            if ((rc = run_call(ctx, h->buf, v, p, sp, acfg, it == 0, norm_mean_dev, norm_sig_dev, rawdp_cap)))
                 return rc;
-            if ((rc = tb2_launch_count_active(ctx, v, P[B_COUNTERS].as<int>()))) return rc;
+            if ((rc = tb2_launch_count_active(ctx, v, h->buf.counters.as<int>()))) return rc;
             if (attempt == 0 && it == 0 && ctx->after_first_launch) {
                 auto fn = std::move(ctx->after_first_launch);
                 ctx->after_first_launch = nullptr;
@@ -491,7 +511,7 @@ static int batch_compute_impl(tb2_ctx *ctx, const tb2_params *params,
                 ctx->pinned_cap = 256;
             }
             const double th0 = trace ? now_ms() : 0;
-            TB2_CUDA_TRY(ctx, cudaMemcpyAsync(ctx->pinned, P[B_COUNTERS].p, 8, cudaMemcpyDeviceToHost, s));
+            TB2_CUDA_TRY(ctx, cudaMemcpyAsync(ctx->pinned, h->buf.counters.p, 8, cudaMemcpyDeviceToHost, s));
             TB2_CUDA_TRY(ctx, cudaStreamSynchronize(s));
             memcpy(counters, ctx->pinned, 8);
             if (trace) fprintf(stderr, "[tb2]   call %d.%d: enqueued at +%.2f ms, synced at +%.2f ms\n", attempt, it, th0 - tc0, now_ms() - tc0);
@@ -505,18 +525,11 @@ static int batch_compute_impl(tb2_ctx *ctx, const tb2_params *params,
     }
     // ---- export into device staging ----
     const size_t nsegs = (size_t)hb.total_b + n;
-    TB2_CUDA_TRY(ctx, P[B_OUT_SEGS].reserve(nsegs * 8 + 8));
-    const size_t small_bytes = (size_t)n * (8 + sizeof(tb2_scale_values) + 8 + 4 + 4 + 4);
-    TB2_CUDA_TRY(ctx, P[B_OUT_SMALL].reserve(small_bytes + 64));
-    unsigned char *sm = P[B_OUT_SMALL].as<unsigned char>();
-    long long *d_rs = (long long *)sm;
-    tb2_scale_values *d_sv = (tb2_scale_values *)(d_rs + n);
-    double *d_score = (double *)(d_sv + n);
-    int *d_status = (int *)(d_score + n);
-    int *d_iters = d_status + n;
-    int *d_flags = d_iters + n;
-    k_export<<<n, 128, 0, s>>>(v, P[B_DBG].as<int>(), P[B_OUT_SEGS].as<long long>(), d_rs, d_sv,
-                               d_score, d_status, d_iters, d_flags);
+    TB2_CUDA_TRY(ctx, h->out_segs.reserve(nsegs * 8 + 8));
+    TB2_CUDA_TRY(ctx, h->out_small.reserve(small_out_bytes(n) + 64));
+    const SmallOut o = small_out(h->out_small, n);
+    k_export<<<n, 128, 0, s>>>(v, h->buf.dbg.as<int>(), h->out_segs.as<long long>(), o.rsrtr, o.sv,
+                               o.score, o.status, o.n_iters, o.flags);
     TB2_CHECK_LAUNCH(ctx);
     TB2_CUDA_TRY(ctx, cudaEventRecord(ctx->ev1, s));
     TB2_CUDA_TRY(ctx, cudaStreamSynchronize(s));
@@ -536,7 +549,7 @@ int tb2_batch_result_view(tb2_ctx *ctx, BatchResultView *out)
     if (!h->computed) { ctx->err = "tb2_batch_compute has not been called"; return TB2_ERR_INVALID_ARG; }
     out->n_reads = h->hb.n;
     out->total_bases = h->hb.total_b;
-    out->norm_mean = ctx->pool[B_OUT_NORMMEAN].as<double>();
+    out->norm_mean = h->out_norm_mean.as<double>();
     out->base_off = h->v.base_off;
     out->seq_off = h->v.seq_off;
     out->seq = h->v.seq;
@@ -559,27 +572,20 @@ static int batch_download_impl(tb2_ctx *ctx, int64_t *segs, int64_t *read_start_
         return TB2_ERR_INVALID_ARG;
     const HostBatch &hb = h->hb;
     const int n = hb.n;
-    auto &P = ctx->pool;
     cudaStream_t s = ctx->stream;
     const size_t nsegs = (size_t)hb.total_b + n;
-    unsigned char *sm = P[B_OUT_SMALL].as<unsigned char>();
-    long long *d_rs = (long long *)sm;
-    tb2_scale_values *d_sv = (tb2_scale_values *)(d_rs + n);
-    double *d_score = (double *)(d_sv + n);
-    int *d_status = (int *)(d_score + n);
-    int *d_iters = d_status + n;
-    int *d_flags = d_iters + n;
-    TB2_CUDA_TRY(ctx, cudaMemcpyAsync(segs, P[B_OUT_SEGS].p, nsegs * 8, cudaMemcpyDeviceToHost, s));
-    TB2_CUDA_TRY(ctx, cudaMemcpyAsync(read_start_rel_to_raw, d_rs, (size_t)n * 8, cudaMemcpyDeviceToHost, s));
-    TB2_CUDA_TRY(ctx, cudaMemcpyAsync(scale_out, d_sv, (size_t)n * sizeof(tb2_scale_values), cudaMemcpyDeviceToHost, s));
-    TB2_CUDA_TRY(ctx, cudaMemcpyAsync(sig_match_score, d_score, (size_t)n * 8, cudaMemcpyDeviceToHost, s));
-    TB2_CUDA_TRY(ctx, cudaMemcpyAsync(status, d_status, (size_t)n * 4, cudaMemcpyDeviceToHost, s));
-    TB2_CUDA_TRY(ctx, cudaMemcpyAsync(n_iters, d_iters, (size_t)n * 4, cudaMemcpyDeviceToHost, s));
-    TB2_CUDA_TRY(ctx, cudaMemcpyAsync(flags, d_flags, (size_t)n * 4, cudaMemcpyDeviceToHost, s));
+    const SmallOut o = small_out(h->out_small, n);
+    TB2_CUDA_TRY(ctx, cudaMemcpyAsync(segs, h->out_segs.p, nsegs * 8, cudaMemcpyDeviceToHost, s));
+    TB2_CUDA_TRY(ctx, cudaMemcpyAsync(read_start_rel_to_raw, o.rsrtr, (size_t)n * 8, cudaMemcpyDeviceToHost, s));
+    TB2_CUDA_TRY(ctx, cudaMemcpyAsync(scale_out, o.sv, (size_t)n * sizeof(tb2_scale_values), cudaMemcpyDeviceToHost, s));
+    TB2_CUDA_TRY(ctx, cudaMemcpyAsync(sig_match_score, o.score, (size_t)n * 8, cudaMemcpyDeviceToHost, s));
+    TB2_CUDA_TRY(ctx, cudaMemcpyAsync(status, o.status, (size_t)n * 4, cudaMemcpyDeviceToHost, s));
+    TB2_CUDA_TRY(ctx, cudaMemcpyAsync(n_iters, o.n_iters, (size_t)n * 4, cudaMemcpyDeviceToHost, s));
+    TB2_CUDA_TRY(ctx, cudaMemcpyAsync(flags, o.flags, (size_t)n * 4, cudaMemcpyDeviceToHost, s));
     if (norm_mean)
-        TB2_CUDA_TRY(ctx, cudaMemcpyAsync(norm_mean, P[B_OUT_NORMMEAN].p, (size_t)hb.total_b * 8, cudaMemcpyDeviceToHost, s));
+        TB2_CUDA_TRY(ctx, cudaMemcpyAsync(norm_mean, h->out_norm_mean.p, (size_t)hb.total_b * 8, cudaMemcpyDeviceToHost, s));
     if (norm_signal)
-        TB2_CUDA_TRY(ctx, cudaMemcpyAsync(norm_signal, P[B_OUT_NORMSIG].p, (size_t)hb.total_s * 8, cudaMemcpyDeviceToHost, s));
+        TB2_CUDA_TRY(ctx, cudaMemcpyAsync(norm_signal, h->out_norm_sig.p, (size_t)hb.total_s * 8, cudaMemcpyDeviceToHost, s));
     if (!ctx->async_mode) TB2_CUDA_TRY(ctx, cudaStreamSynchronize(s));
     return TB2_OK;
 }
@@ -740,34 +746,43 @@ static int resquiggle_batch_impl(tb2_ctx *ctx, int64_t n_reads, const void *raw,
 // ---------------------------------------------------------------------------
 namespace {
 
-// a one-read view over caller supplied signal; no sequence / model needed
+// a one-read view over caller supplied signal; no sequence / model needed.  It lives in the
+// context's single-read buffer set, never in the resident batch's.
 struct OneRead {
     HostBatch hb;
     BatchView v;
     int64_t raw_off[2], seq_off[2];
+    BatchBuffers *buf;
 };
 
+ReadState active_read()
+{
+    ReadState st;
+    memset(&st, 0, sizeof(st));
+    st.active = 1;
+    return st;
+}
+
+// st: the read's initial state
 int one_read_view(tb2_ctx *ctx, OneRead &o, const double *sig, int64_t n, int64_t nb,
-                  const tb2_params &p, int64_t ev_cap)
+                  const tb2_params &p, int64_t ev_cap, const ReadState &st)
 {
     o.raw_off[0] = 0; o.raw_off[1] = n;
     o.seq_off[0] = 0; o.seq_off[1] = nb;   // K = 1
-    int rc = build_view(ctx, 1, o.raw_off, o.seq_off, 1, p, 1.1, 0, o.hb, o.v);
+    o.buf = &tb2_state(ctx->one_read);
+    int rc = build_view(ctx, *o.buf, 1, o.raw_off, o.seq_off, 1, p, 1.1, 0, o.hb, o.v);
     if (rc) return rc;
     if (ev_cap + 2 > o.hb.ev_off[1]) {
         // enlarge the event slots
         o.hb.ev_off[1] = ev_cap + 2;
-        TB2_CUDA_TRY(ctx, ctx->pool[B_CPTS].reserve((size_t)(ev_cap + 2) * 4 + 8));
-        TB2_CUDA_TRY(ctx, ctx->pool[B_EM].reserve((size_t)(ev_cap + 2) * 8 + 8));
-        o.v.cpts = ctx->pool[B_CPTS].as<int>();
-        o.v.em = ctx->pool[B_EM].as<double>();
-        TB2_CUDA_TRY(ctx, cudaMemcpyAsync(ctx->pool[B_EVOFF].p, o.hb.ev_off.data(), 16, cudaMemcpyHostToDevice, ctx->stream));
+        TB2_CUDA_TRY(ctx, o.buf->cpts.reserve((size_t)(ev_cap + 2) * 4 + 8));
+        TB2_CUDA_TRY(ctx, o.buf->em.reserve((size_t)(ev_cap + 2) * 8 + 8));
+        o.v.cpts = o.buf->cpts.as<int>();
+        o.v.em = o.buf->em.as<double>();
+        TB2_CUDA_TRY(ctx, cudaMemcpyAsync(o.buf->ev_off.p, o.hb.ev_off.data(), 16, cudaMemcpyHostToDevice, ctx->stream));
     }
     if (sig)
         TB2_CUDA_TRY(ctx, cudaMemcpyAsync(o.v.rawf, sig, (size_t)n * 8, cudaMemcpyHostToDevice, ctx->stream));
-    ReadState st;
-    memset(&st, 0, sizeof(st));
-    st.active = 1;
     TB2_CUDA_TRY(ctx, cudaMemcpyAsync(o.v.st, &st, sizeof(st), cudaMemcpyHostToDevice, ctx->stream));
     return TB2_OK;
 }
@@ -810,13 +825,10 @@ extern "C" int tb2_normalize_raw_signal(tb2_ctx *ctx, const double *raw, int64_t
     if (rc) return rc;
     if (!raw || !norm_out || !sv_out || n < 1 || (norm_type != 0 && norm_type != 1))
         return TB2_ERR_INVALID_ARG;
-    OneRead o;
-    if ((rc = one_read_view(ctx, o, raw, n, 1, default_params(), 2))) return rc;
-    ReadState st;
-    memset(&st, 0, sizeof(st));
-    st.active = 1;
+    ReadState st = active_read();
     if (sv_in) { st.use_sv = 1; st.sv = *sv_in; }
-    TB2_CUDA_TRY(ctx, cudaMemcpyAsync(o.v.st, &st, sizeof(st), cudaMemcpyHostToDevice, ctx->stream));
+    OneRead o;
+    if ((rc = one_read_view(ctx, o, raw, n, 1, default_params(), 2, st))) return rc;
     StagePolicy sp;
     memset(&sp, 0, sizeof(sp));
     sp.outlier_thresh = outlier_thresh;
@@ -842,13 +854,10 @@ extern "C" int tb2_valid_cpts_w_cap(tb2_ctx *ctx, const double *sig, int64_t n,
     p.min_obs_per_base = min_base_obs;
     p.running_stat_width = running_stat_width;
     p.use_t_test_seg = t_test ? 1 : 0;
-    OneRead o;
-    if ((rc = one_read_view(ctx, o, sig, n, 1, p, num_cpts))) return rc;
-    ReadState st;
-    memset(&st, 0, sizeof(st));
-    st.active = 1;
+    ReadState st = active_read();
     st.num_events = (int)num_cpts;
-    TB2_CUDA_TRY(ctx, cudaMemcpyAsync(o.v.st, &st, sizeof(st), cudaMemcpyHostToDevice, ctx->stream));
+    OneRead o;
+    if ((rc = one_read_view(ctx, o, sig, n, 1, p, num_cpts, st))) return rc;
     if ((rc = tb2_launch_cpts(ctx, o.v, p, 1))) return rc;
     if ((rc = fetch_state(ctx, o.v, &st))) return rc;
     if (read_status) *read_status = st.status;
@@ -866,8 +875,10 @@ extern "C" int tb2_new_means(tb2_ctx *ctx, const double *sig, int64_t n_sig, con
     int rc = tb2_use(ctx);
     if (rc) return rc;
     if (!sig || !segs || !means_out || n_sig < 1 || n_segs < 1) return TB2_ERR_INVALID_ARG;
+    ReadState st = active_read();
+    st.n_cpts = (int)n_segs + 1;
     OneRead o;
-    if ((rc = one_read_view(ctx, o, nullptr, n_sig, 1, default_params(), n_segs + 1))) return rc;
+    if ((rc = one_read_view(ctx, o, nullptr, n_sig, 1, default_params(), n_segs + 1, st))) return rc;
     // event means kernel reads `norm`
     TB2_CUDA_TRY(ctx, cudaMemcpyAsync(o.v.norm, sig, (size_t)n_sig * 8, cudaMemcpyHostToDevice, ctx->stream));
     std::vector<int> s32((size_t)n_segs + 1);
@@ -876,11 +887,6 @@ extern "C" int tb2_new_means(tb2_ctx *ctx, const double *sig, int64_t n_sig, con
         s32[i] = (int)segs[i];
     }
     TB2_CUDA_TRY(ctx, cudaMemcpyAsync(o.v.cpts, s32.data(), (size_t)(n_segs + 1) * 4, cudaMemcpyHostToDevice, ctx->stream));
-    ReadState st;
-    memset(&st, 0, sizeof(st));
-    st.active = 1;
-    st.n_cpts = (int)n_segs + 1;
-    TB2_CUDA_TRY(ctx, cudaMemcpyAsync(o.v.st, &st, sizeof(st), cudaMemcpyHostToDevice, ctx->stream));
     if ((rc = tb2_launch_event_means(ctx, o.v))) return rc;
     TB2_CUDA_TRY(ctx, cudaMemcpyAsync(means_out, o.v.em, (size_t)n_segs * 8, cudaMemcpyDeviceToHost, ctx->stream));
     TB2_CUDA_TRY(ctx, cudaStreamSynchronize(ctx->stream));
@@ -894,16 +900,13 @@ extern "C" int tb2_theil_sen(tb2_ctx *ctx, double prev_shift, double prev_scale,
     int rc = tb2_use(ctx);
     if (rc) return rc;
     if (!event_means || !model_means || !out4 || n < 1) return TB2_ERR_INVALID_ARG;
+    ReadState st = active_read();
+    st.sv.shift = prev_shift; st.sv.scale = prev_scale;
     OneRead o;
     // K = 1: seq_off = n gives n mapped bases
-    if ((rc = one_read_view(ctx, o, nullptr, 1, n, default_params(), 2))) return rc;
+    if ((rc = one_read_view(ctx, o, nullptr, 1, n, default_params(), 2, st))) return rc;
     TB2_CUDA_TRY(ctx, cudaMemcpyAsync(o.v.bm, event_means, (size_t)n * 8, cudaMemcpyHostToDevice, ctx->stream));
     TB2_CUDA_TRY(ctx, cudaMemcpyAsync(o.v.rm, model_means, (size_t)n * 8, cudaMemcpyHostToDevice, ctx->stream));
-    ReadState st;
-    memset(&st, 0, sizeof(st));
-    st.active = 1;
-    st.sv.shift = prev_shift; st.sv.scale = prev_scale;
-    TB2_CUDA_TRY(ctx, cudaMemcpyAsync(o.v.st, &st, sizeof(st), cudaMemcpyHostToDevice, ctx->stream));
     StagePolicy sp;
     memset(&sp, 0, sizeof(sp));
     sp.outlier_thresh = NAN;
@@ -929,7 +932,7 @@ extern "C" int tb2_resolve_skipped_bases_with_raw(tb2_ctx *ctx, const int64_t *s
         n_norm < 1)
         return TB2_ERR_INVALID_ARG;
     OneRead o;
-    if ((rc = one_read_view(ctx, o, nullptr, n_norm, n_bases, default_params(), 2))) return rc;
+    if ((rc = one_read_view(ctx, o, nullptr, n_norm, n_bases, default_params(), 2, active_read()))) return rc;
     cudaStream_t s = ctx->stream;
     TB2_CUDA_TRY(ctx, cudaMemcpyAsync(o.v.norm, norm_signal, (size_t)n_norm * 8, cudaMemcpyHostToDevice, s));
     TB2_CUDA_TRY(ctx, cudaMemcpyAsync(o.v.rm, ref_means, (size_t)n_bases * 8, cudaMemcpyHostToDevice, s));
@@ -937,14 +940,11 @@ extern "C" int tb2_resolve_skipped_bases_with_raw(tb2_ctx *ctx, const int64_t *s
     std::vector<int> s32((size_t)n_bases + 1);
     for (int64_t i = 0; i <= n_bases; ++i) s32[i] = (int)segs[i];
     TB2_CUDA_TRY(ctx, cudaMemcpyAsync(o.v.segs_dp, s32.data(), (size_t)(n_bases + 1) * 4, cudaMemcpyHostToDevice, s));
-    ReadState st;
-    memset(&st, 0, sizeof(st));
-    st.active = 1;
-    TB2_CUDA_TRY(ctx, cudaMemcpyAsync(o.v.st, &st, sizeof(st), cudaMemcpyHostToDevice, s));
     StagePolicy sp;
     memset(&sp, 0, sizeof(sp));
     sp.max_raw_cpts = max_raw_cpts;
     if ((rc = tb2_launch_resolve(ctx, o.v, *params, sp, (size_t)1 << 20))) return rc;
+    ReadState st;
     if ((rc = fetch_state(ctx, o.v, &st))) return rc;
     if (read_status) *read_status = st.status;
     if (st.status == TB2_OK) {
@@ -961,11 +961,10 @@ extern "C" int tb2_identify_stalls(tb2_ctx *ctx, const double *raw, int64_t n, i
     if (rc) return rc;
     if (!raw || !ints_out || !n_out || n < 1 || cap < 1) return TB2_ERR_INVALID_ARG;
     OneRead o;
-    if ((rc = one_read_view(ctx, o, raw, n, 1, default_params(), 2))) return rc;
-    auto &P = ctx->pool;
+    if ((rc = one_read_view(ctx, o, raw, n, 1, default_params(), 2, active_read()))) return rc;
     const int scap = 4096;
-    TB2_CUDA_TRY(ctx, P[B_STALLS].reserve((size_t)2 * scap * 4));
-    o.v.stall_ints = P[B_STALLS].as<int>();
+    TB2_CUDA_TRY(ctx, o.buf->stalls.reserve((size_t)2 * scap * 4));
+    o.v.stall_ints = o.buf->stalls.as<int>();
     o.v.stall_cap = scap;
     if ((rc = tb2_launch_stalls(ctx, o.v))) return rc;
     ReadState st;

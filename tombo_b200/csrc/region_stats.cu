@@ -22,16 +22,20 @@
 #include <vector>
 
 namespace {
-enum { R_CNT = 80, R_STAT, R_POS, R_OUT_POS, R_OUT_F, R_OUT_D, R_OUT_C, R_OUT_V, R_SCAN, R_N,
-       F_MEAN, F_RM, F_RS, F_OFF, F_OUT, F_LOGP, F_SEQ, F_SOFF, F_START, F_POS, F_SOFFOUT };
+// per-call scratch of the entry points below; nothing reads it after a call returns
+enum { R_STAT = 0, R_POS, R_OUT_POS, R_OUT_F, R_OUT_D, R_OUT_C, R_OUT_V, R_N,
+       F_MEAN, F_RM, F_RS, F_OFF, F_OUT, F_LOGP, F_SEQ, F_SOFF, F_START, F_POS, RS_COUNT };
+}  // namespace
 
-struct RegionState { long long start = 0, len = 0; bool open = false; };
-RegionState &region_of(tb2_ctx *ctx)
-{
-    if (!ctx->region) ctx->region = std::shared_ptr<void>(new RegionState(), [](void *p) { delete (RegionState *)p; });
-    return *(RegionState *)ctx->region.get();
-}
+struct RegionState {
+    // the open region and its counters: 3 * len ints, then the out-of-region count
+    long long start = 0, len = 0;
+    bool open = false;
+    DevBuf cnt;
+    DevBuf scratch[RS_COUNT];
+};
 
+namespace {
 // stat_type 0: alternative-model LLRs (|stat| >= thresh is "valid" when no lower
 // threshold is given, apply_per_read_thresh :4099-4105); 1: everything else
 __global__ void k_region_accumulate(long long n, const double *stats, const long long *pos,
@@ -108,9 +112,9 @@ extern "C" int tb2_region_stats_begin(tb2_ctx *ctx, int64_t reg_start, int64_t r
     int rc = tb2_use(ctx);
     if (rc) return rc;
     if (reg_len < 1 || reg_len > (1LL << 28)) return TB2_ERR_INVALID_ARG;
-    RegionState &rs = region_of(ctx);
-    TB2_CUDA_TRY(ctx, ctx->pool[R_CNT].reserve((size_t)reg_len * 3 * 4 + 16));
-    TB2_CUDA_TRY(ctx, cudaMemsetAsync(ctx->pool[R_CNT].p, 0, (size_t)reg_len * 3 * 4 + 16, ctx->stream));
+    RegionState &rs = tb2_state(ctx->region);
+    TB2_CUDA_TRY(ctx, rs.cnt.reserve((size_t)reg_len * 3 * 4 + 16));
+    TB2_CUDA_TRY(ctx, cudaMemsetAsync(rs.cnt.p, 0, (size_t)reg_len * 3 * 4 + 16, ctx->stream));
     rs.start = reg_start; rs.len = reg_len; rs.open = true;
     return TB2_OK;
 }
@@ -119,10 +123,10 @@ extern "C" int tb2_region_stats_begin(tb2_ctx *ctx, int64_t reg_start, int64_t r
 int tb2_region_accumulate_dev(tb2_ctx *ctx, long long n, const double *stats_dev,
                               const long long *pos_dev, double thresh, double lower, int stat_type)
 {
-    RegionState &rs = region_of(ctx);
+    RegionState &rs = tb2_state(ctx->region);
     if (!rs.open) { ctx->err = "tb2_region_stats_begin has not been called"; return TB2_ERR_INVALID_ARG; }
     if (n <= 0) return TB2_OK;
-    int *cnt = ctx->pool[R_CNT].as<int>();
+    int *cnt = rs.cnt.as<int>();
     k_region_accumulate<<<(unsigned)((n + 255) / 256), 256, 0, ctx->stream>>>(
         n, stats_dev, pos_dev, rs.start, rs.len, thresh, lower, stat_type, cnt,
         (unsigned long long *)(cnt + 3 * rs.len + ((3 * rs.len) & 1)));
@@ -137,7 +141,7 @@ extern "C" int tb2_region_stats_add(tb2_ctx *ctx, int64_t n, const double *stats
     if (rc) return rc;
     if (n < 0 || (n > 0 && (!stats || !pos)) || isnan(single_read_thresh)) return TB2_ERR_INVALID_ARG;
     if (n == 0) return TB2_OK;
-    auto &P = ctx->pool;
+    auto &P = tb2_state(ctx->region).scratch;
     TB2_CUDA_TRY(ctx, P[R_STAT].reserve((size_t)n * 8));
     TB2_CUDA_TRY(ctx, P[R_POS].reserve((size_t)n * 8));
     TB2_CUDA_TRY(ctx, cudaMemcpyAsync(P[R_STAT].p, stats, (size_t)n * 8, cudaMemcpyHostToDevice, ctx->stream));
@@ -153,9 +157,9 @@ extern "C" int tb2_region_counts_get(tb2_ctx *ctx, int32_t *counts)
 {
     int rc = tb2_use(ctx);
     if (rc) return rc;
-    RegionState &rs = region_of(ctx);
+    RegionState &rs = tb2_state(ctx->region);
     if (!rs.open || !counts) return TB2_ERR_INVALID_ARG;
-    TB2_CUDA_TRY(ctx, cudaMemcpyAsync(counts, ctx->pool[R_CNT].p, (size_t)rs.len * 3 * 4, cudaMemcpyDeviceToHost, ctx->stream));
+    TB2_CUDA_TRY(ctx, cudaMemcpyAsync(counts, rs.cnt.p, (size_t)rs.len * 3 * 4, cudaMemcpyDeviceToHost, ctx->stream));
     TB2_CUDA_TRY(ctx, cudaStreamSynchronize(ctx->stream));
     return TB2_OK;
 }
@@ -164,9 +168,9 @@ extern "C" int tb2_region_counts_set(tb2_ctx *ctx, const int32_t *counts)
 {
     int rc = tb2_use(ctx);
     if (rc) return rc;
-    RegionState &rs = region_of(ctx);
+    RegionState &rs = tb2_state(ctx->region);
     if (!rs.open || !counts) return TB2_ERR_INVALID_ARG;
-    TB2_CUDA_TRY(ctx, cudaMemcpyAsync(ctx->pool[R_CNT].p, counts, (size_t)rs.len * 3 * 4, cudaMemcpyHostToDevice, ctx->stream));
+    TB2_CUDA_TRY(ctx, cudaMemcpyAsync(rs.cnt.p, counts, (size_t)rs.len * 3 * 4, cudaMemcpyHostToDevice, ctx->stream));
     TB2_CUDA_TRY(ctx, cudaStreamSynchronize(ctx->stream));
     return TB2_OK;
 }
@@ -178,10 +182,10 @@ extern "C" int tb2_region_stats_finalize(tb2_ctx *ctx, double unmod_count, doubl
 {
     int rc = tb2_use(ctx);
     if (rc) return rc;
-    RegionState &rs = region_of(ctx);
+    RegionState &rs = tb2_state(ctx->region);
     if (!rs.open || cap < 0 || !n_out || (cap > 0 && (!pos_out || !frac_out || !damp_frac_out || !cov_out || !valid_cov_out)))
         return TB2_ERR_INVALID_ARG;
-    auto &P = ctx->pool;
+    auto &P = rs.scratch;
     cudaStream_t s = ctx->stream;
     const size_t c = (size_t)std::min<long long>(cap, rs.len);
     TB2_CUDA_TRY(ctx, P[R_OUT_POS].reserve(c * 8 + 8));
@@ -190,7 +194,7 @@ extern "C" int tb2_region_stats_finalize(tb2_ctx *ctx, double unmod_count, doubl
     TB2_CUDA_TRY(ctx, P[R_OUT_C].reserve(c * 8 + 8));
     TB2_CUDA_TRY(ctx, P[R_OUT_V].reserve(c * 8 + 8));
     TB2_CUDA_TRY(ctx, P[R_N].reserve(8));
-    k_region_finalize<<<1, 1024, 0, s>>>(P[R_CNT].as<int>(), rs.start, rs.len, unmod_count, mod_count,
+    k_region_finalize<<<1, 1024, 0, s>>>(rs.cnt.as<int>(), rs.start, rs.len, unmod_count, mod_count,
                                          (long long)c, P[R_OUT_POS].as<long long>(), P[R_OUT_F].as<double>(),
                                          P[R_OUT_D].as<double>(), P[R_OUT_C].as<long long>(),
                                          P[R_OUT_V].as<long long>(), P[R_N].as<long long>());
@@ -217,7 +221,7 @@ extern "C" int tb2_region_stats_finalize(tb2_ctx *ctx, double unmod_count, doubl
 static int fisher_common(tb2_ctx *ctx, FisherArgs &a, int n_segs, long long total, bool kmer,
                          double *pvals_out, int64_t *pos_out)
 {
-    auto &P = ctx->pool;
+    auto &P = tb2_state(ctx->region).scratch;
     cudaStream_t s = ctx->stream;
     TB2_CUDA_TRY(ctx, P[F_OUT].reserve((size_t)total * 8 + 8));
     TB2_CUDA_TRY(ctx, P[F_LOGP].reserve((size_t)total * 8 + 8));
@@ -255,7 +259,7 @@ extern "C" int tb2_window_fisher_pvals(tb2_ctx *ctx, int64_t n_segs, const doubl
     const bool is_p = !ref_means && !ref_sds;           // p-values in, Fisher window only
     if (total < 0 || seg_off[0] != 0 || (total > 0 && (!means || !pvals_out)) || (!ref_means != !ref_sds))
         return TB2_ERR_INVALID_ARG;
-    auto &P = ctx->pool;
+    auto &P = tb2_state(ctx->region).scratch;
     cudaStream_t s = ctx->stream;
     TB2_CUDA_TRY(ctx, P[F_MEAN].reserve((size_t)total * 8 + 8));
     TB2_CUDA_TRY(ctx, P[F_RM].reserve((size_t)total * 8 + 8));
@@ -297,7 +301,7 @@ extern "C" int tb2_de_novo_read_stats_batch(tb2_ctx *ctx, int64_t n_reads, const
     }
     const long long total = stat_off[n];
     if (total > 0 && (!norm_mean || !seq || !pvals_out || !pos_out)) return TB2_ERR_INVALID_ARG;
-    auto &P = ctx->pool;
+    auto &P = tb2_state(ctx->region).scratch;
     cudaStream_t s = ctx->stream;
     const size_t tm = (size_t)mean_off[n], ts = (size_t)seq_off[n];
     TB2_CUDA_TRY(ctx, P[F_MEAN].reserve(tm * 8 + 8));

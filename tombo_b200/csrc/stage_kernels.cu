@@ -1,5 +1,6 @@
 // stage_kernels.cu -- launch wrappers of the stage kernels (device code: stage_kernels.cuh)
 #include "stage_kernels.cuh"
+#include "kernels.h"
 
 // ===========================================================================
 // launch wrappers
@@ -98,25 +99,24 @@ int tb2_launch_stalls(tb2_ctx *ctx, const BatchView &b)
 int tb2_launch_resolve(tb2_ctx *ctx, const BatchView &b, const tb2_params &p,
                        const StagePolicy &pol, size_t cap)
 {
-    enum { SLOT_RAWDP = 73, SLOT_CNT2 = 74, SLOT_RAWBIG = 75 };
     const int warps_per_block = 4;
     int grid = ctx->sm_count * 8;
     const int max_useful = (b.n_reads + warps_per_block - 1) / warps_per_block;
     if (grid > max_useful) grid = max_useful > 0 ? max_useful : 1;
     const size_t slots = (size_t)grid * warps_per_block;
-    TB2_CUDA_TRY(ctx, ctx->pool[SLOT_RAWDP].reserve(slots * cap * sizeof(double)));
-    TB2_CUDA_TRY(ctx, ctx->pool[SLOT_CNT2].reserve(16));
-    TB2_CUDA_TRY(ctx, cudaMemsetAsync(ctx->pool[SLOT_CNT2].p, 0, 16, ctx->stream));
+    LaunchScratch &ls = tb2_state(ctx->launch_scratch);
+    TB2_CUDA_TRY(ctx, ls.raw_dp.reserve(slots * cap * sizeof(double)));
+    TB2_CUDA_TRY(ctx, ls.resolve_cnt.reserve(16));
+    TB2_CUDA_TRY(ctx, cudaMemsetAsync(ls.resolve_cnt.p, 0, 16, ctx->stream));
     // overflow arena for windows beyond the per-warp slab: a window is at most
     // (2 * MAX_DEL_FIX_WINDOW + few) bases x its samples; sized from the longest read,
     // 64 MB .. 2 GB
     const unsigned long long big_cap = std::min<unsigned long long>(
         (2ULL << 30) / 8, std::max<unsigned long long>((64ULL << 20) / 8, 24ULL * 64ULL * (unsigned long long)std::max(1, b.max_raw)));
-    TB2_CUDA_TRY(ctx, ctx->pool[SLOT_RAWBIG].reserve((size_t)big_cap * sizeof(double)));
+    TB2_CUDA_TRY(ctx, ls.raw_big.reserve((size_t)big_cap * sizeof(double)));
     k_resolve<<<grid, warps_per_block * 32, 0, ctx->stream>>>(
-        b, p, pol, ctx->pool[SLOT_RAWDP].as<double>(), cap, ctx->pool[SLOT_CNT2].as<int>(),
-        ctx->pool[SLOT_RAWBIG].as<double>(), big_cap,
-        (unsigned long long *)(ctx->pool[SLOT_CNT2].as<int>() + 2));
+        b, p, pol, ls.raw_dp.as<double>(), cap, ls.resolve_cnt.as<int>(), ls.raw_big.as<double>(),
+        big_cap, (unsigned long long *)(ls.resolve_cnt.as<int>() + 2));
     TB2_CHECK_LAUNCH(ctx);
     return TB2_OK;
 }
