@@ -17,7 +17,7 @@
  *     _c_dynamic_programming.pyx:9-13, _c_helper.pyx:6-13).
  *   - every call returns 0 (TB2_OK) or a TB2_ERR_* code; per-read outcomes of
  *     batched calls are reported in a status array with the same codes.  Codes
- *     1..21 map 1:1 onto the reference's TomboError / NotImplementedError message
+ *     1..22 map 1:1 onto the reference's TomboError / NotImplementedError message
  *     strings (tb2_status_message); the reference raises, we return.
  *   - there is NO CPU fallback: every entry point runs CUDA kernels and fails with
  *     TB2_ERR_CUDA if no sm_90-class device is usable.
@@ -55,6 +55,7 @@ enum {
     TB2_ERR_SEG_COUNT = 19,             /* resquiggle.py:1201 */
     TB2_ERR_THEIL_SEN_ZERO = 20,        /* tombo_stats.py:421 */
     TB2_ERR_INVALID_START_PATH = 21,    /* tombo_stats.py:2356 */
+    TB2_ERR_READ_TOO_SHORT_IN_REGION = 22,  /* tombo_stats.py:3944 */
     TB2_ERR_UNEXPECTED = 100,  /* the reference would raise a non-Tombo exception */
     /* library level */
     TB2_ERR_CUDA = 200,        /* CUDA runtime failure (see tb2_last_error) */
@@ -96,6 +97,14 @@ typedef struct tb2_policy {
 } tb2_policy;
 
 typedef struct tb2_ctx tb2_ctx;
+
+/* a TomboMotif (tombo_helper.py:542-640): mask[j] is the IUPAC class of motif base j as a
+ * bit set (A = 1, C = 2, G = 4, T = 8; 'N' = 15), 1 <= len <= 32, 1-based
+ * 1 <= mod_pos <= len; no mask may be 0 */
+typedef struct tb2_motif {
+    int32_t len, mod_pos;
+    uint8_t mask[32];
+} tb2_motif;
 
 /* ---- context ---------------------------------------------------------- */
 int tb2_abi_version(void);
@@ -286,7 +295,8 @@ int tb2_batch_download(tb2_ctx *ctx, int64_t *segs, int64_t *read_start_rel_to_r
  * Sites are the positions of `alt_base_code` in the motif-searchable part of each
  * read (single-base motif, TomboMotif(alt_base, 1)).  site_off has n_reads+1
  * entries (filled); llr_out / pos_out sized by the caller to site capacity
- * (sum of n_bases is always enough). */
+ * (sum of n_bases is always enough).  Motif models, '-' strand reads and regions:
+ * tb2_alt_model_llr_motif_batch. */
 int tb2_alt_model_llr_batch(
     tb2_ctx *ctx, int64_t n_reads, const double *norm_mean,
     const int64_t *mean_off, const uint8_t *seq, const int64_t *seq_off,
@@ -317,11 +327,57 @@ int tb2_timer_stop(tb2_ctx *ctx, double *ms_out);
  * are already there.  read_start[n_reads] are the reads' genome start positions.  LLRs and
  * positions stay on the device for tb2_region_stats_add_batch_llr; tb2_batch_llr_download
  * copies them out (site_off has n_reads + 1 entries; llr_out / pos_out sized
- * *n_sites_total). */
+ * *n_sites_total).  Single-base motif, whole '+' strand reads; any motif, both strands and
+ * a region: tb2_batch_alt_llr_motif. */
 int tb2_batch_alt_llr(tb2_ctx *ctx, const int64_t *read_start, int alt_base_code,
                       int use_standard_llhr, double scale_factor, double height_factor,
                       double height_power, int64_t *n_sites_total);
 int tb2_batch_llr_download(tb2_ctx *ctx, double *llr_out, int64_t *pos_out, int64_t *site_off);
+
+/* ---- alternative-model LLRs for any motif, both strands, one region ------------------
+ * compute_alt_model_read_stats (tombo_stats.py:3972-4082) with trim_seq_and_means
+ * (:3888-3970) for one alt model with a motif (tombo.DNA.CpG / dam / dcm: CG:1, GATC:2,
+ * CCWGG:2), reads mapped to either strand and the region [reg_start, reg_end).  The data
+ * are read-centric as the reference stores them: read r's nb trimmed bases S (the reverse
+ * complement of the genome for '-' reads) sit at seq[seq_off[r] + cpos ...] inside its
+ * nb + K - 1 codes, with the nb per-base means; read_start[r] is the genome's low
+ * coordinate on both strands.  Codes outside S are read as 'N' whatever they hold.
+ *   - strand[r]: 0 '+', 1 '-', -1 skip the read (no sites, status 0; on the resident
+ *     batch a read whose resquiggle failed reports that status whatever its strand).
+ *   - max_motif_bb / max_motif_ab: max(mod_pos - 1) and max(len - mod_pos) over every alt
+ *     model of the reference's call, so several calls (one per model) reproduce one joint
+ *     call; each must be at least this motif's own value.
+ *   - reads that reach outside the region are clipped as the reference does; a read with
+ *     fewer than K testable levels left gets TB2_ERR_READ_TOO_SHORT_IN_REGION in
+ *     read_status (nullable, n_reads entries; 0 otherwise) and no sites.  A region that
+ *     contains every read ([min start, max start + nb)) scores whole reads (reg_data=None).
+ *   - sites are the leftmost non-overlapping motif matches (re.finditer) in read order;
+ *     positions are genome positions, descending for '-' reads, as the reference returns
+ *     them.
+ *   - the reference's zero-width slice quirks are kept: with central_pos == K - 1 every
+ *     read whose 3' end is not clipped is too short, and when clip3 + K - 1 == max_ab
+ *     (e.g. CNNNNN:1 with 6-mers on a whole read) the read has no sites.
+ * TB2_ERR_INVALID_ARG: malformed motif, max_motif_bb < mod_pos - 1, max_motif_ab <
+ * len - mod_pos, a strand outside {-1, 0, 1}, models of different k-mer widths, or reads
+ * whose code count is not nb + K - 1.  llr_out / pos_out hold up to sum(nb) sites. */
+int tb2_alt_model_llr_motif_batch(
+    tb2_ctx *ctx, int64_t n_reads, const double *norm_mean, const int64_t *mean_off,
+    const uint8_t *seq, const int64_t *seq_off, const int64_t *read_start, const int8_t *strand,
+    const tb2_motif *motif, int64_t max_motif_bb, int64_t max_motif_ab, int64_t reg_start,
+    int64_t reg_end, int use_standard_llhr, double scale_factor, double height_factor,
+    double height_power, double *llr_out, int64_t *pos_out, int64_t *site_off,
+    int32_t *read_status);
+/* the same on the RESIDENT batch (after tb2_batch_compute); read_start / strand have
+ * n_reads entries.  It replaces the resident LLRs exactly as tb2_batch_alt_llr does, so
+ * tb2_batch_llr_download and tb2_region_stats_add_batch_llr read its sites: one call per
+ * strand (the other strand's reads at -1) feeds that strand's region counters.  Reads whose
+ * resquiggle failed hold no sites and report their resquiggle status in read_status, also
+ * when their strand is -1. */
+int tb2_batch_alt_llr_motif(tb2_ctx *ctx, const int64_t *read_start, const int8_t *strand,
+                            const tb2_motif *motif, int64_t max_motif_bb, int64_t max_motif_ab,
+                            int64_t reg_start, int64_t reg_end, int use_standard_llhr,
+                            double scale_factor, double height_factor, double height_power,
+                            int32_t *read_status, int64_t *n_sites_total);
 
 /* ---- SURVEY 8(f)-1: per-position aggregation of per-read statistics -----------------
  * collate_reg_stats tombo_stats.py:4124-4178 + apply_per_read_thresh :4084-4122 +

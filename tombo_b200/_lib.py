@@ -45,6 +45,27 @@ class Policy(C.Structure):
                 ('subsample_seed', C.c_uint32), ('rescue', C.c_uint32)]
 
 
+class Motif(C.Structure):
+    """tb2_motif: a TomboMotif as IUPAC bit sets (A = 1, C = 2, G = 4, T = 8)"""
+    _fields_ = [('len', C.c_int32), ('mod_pos', C.c_int32), ('mask', C.c_uint8 * 32)]
+
+
+_IUPAC_BITS = {'A': 1, 'C': 2, 'G': 4, 'T': 8, 'B': 14, 'D': 13, 'H': 11, 'K': 12, 'M': 3,
+               'N': 15, 'R': 5, 'S': 6, 'V': 7, 'W': 9, 'Y': 10}
+
+
+def motif_struct(motif):
+    """tombo_helper.TomboMotif (raw_motif, mod_pos) -> tb2_motif"""
+    raw = motif.raw_motif
+    if not 1 <= len(raw) <= 32 or motif.mod_pos is None:
+        raise ValueError('motifs of 1 to 32 bases with a modified position only')
+    m = Motif()
+    m.len, m.mod_pos = len(raw), int(motif.mod_pos)
+    for j, letter in enumerate(raw):
+        m.mask[j] = _IUPAC_BITS[letter]
+    return m
+
+
 _lib = None
 _lock = threading.Lock()
 
@@ -325,6 +346,7 @@ class Context(object):
         assert means.shape[0] == 4 ** kmer_width == sds.shape[0]
         fn = self.lib.tb2_set_model
         fn.restype = C.c_int
+        self._model_ref = self._model_digest = None     # ensure_model uploads next time
         self.check(fn(self.handle, ptr(means, f64), ptr(sds, f64),
                       C.c_int(kmer_width), C.c_int(central_pos)))
         self.kmer_width, self.central_pos = kmer_width, central_pos
@@ -579,6 +601,57 @@ class Context(object):
         self._llr_total, self._llr_reads = int(tot.value), read_start.shape[0]
         return self._llr_total
 
+    def alt_model_llr_motif_batch(self, norm_mean, mean_off, seq, seq_off, read_start, strand,
+                                  motif, max_motif_bb, max_motif_ab, reg_start, reg_end,
+                                  use_standard_llhr=False, scale_factor=4.0, height_factor=1.0,
+                                  height_power=0.2):
+        """tb2_alt_model_llr_motif_batch; motif is a Motif.  Returns (llr, pos, site_off,
+        read_status)."""
+        norm_mean, mean_off = as_f64(norm_mean), as_i64(mean_off)
+        seq = np.ascontiguousarray(seq, dtype=np.uint8)
+        seq_off, read_start = as_i64(seq_off), as_i64(read_start)
+        strand = np.ascontiguousarray(strand, dtype=np.int8)
+        n = mean_off.shape[0] - 1
+        cap = max(1, norm_mean.shape[0])
+        llr = np.empty(cap)
+        pos = np.empty(cap, dtype=np.int64)
+        site_off = np.zeros(n + 1, dtype=np.int64)
+        status = np.zeros(max(1, n), dtype=np.int32)
+        fn = self.lib.tb2_alt_model_llr_motif_batch
+        fn.restype = C.c_int
+        self.check(fn(self.handle, i64(n), ptr(norm_mean, f64), ptr(mean_off, i64),
+                      ptr(seq, C.c_uint8), ptr(seq_off, i64), ptr(read_start, i64),
+                      ptr(strand, C.c_int8), C.byref(motif), i64(int(max_motif_bb)),
+                      i64(int(max_motif_ab)), i64(int(reg_start)), i64(int(reg_end)),
+                      C.c_int(int(bool(use_standard_llhr))), f64(scale_factor),
+                      f64(height_factor), f64(height_power), ptr(llr, f64), ptr(pos, i64),
+                      ptr(site_off, i64), ptr(status, C.c_int32)))
+        tot = int(site_off[-1])
+        return llr[:tot].copy(), pos[:tot].copy(), site_off, status[:n].copy()
+
+    def batch_alt_llr_motif(self, read_start, strand, motif, max_motif_bb, max_motif_ab,
+                            reg_start, reg_end, use_standard_llhr=False, scale_factor=4.0,
+                            height_factor=1.0, height_power=0.2):
+        """motif LLRs of the resident batch (after batch_compute); returns (site count,
+        read_status).  batch_llr_download and region_stats_add_batch_llr read them."""
+        read_start = as_i64(read_start)
+        strand = np.ascontiguousarray(strand, dtype=np.int8)
+        n = self._base_off.shape[0] - 1 if getattr(self, '_base_off', None) is not None else -1
+        if read_start.shape != (n,) or strand.shape != (n,):
+            raise ValueError('read_start and strand need one entry per read of the resident '
+                             'batch (%d)' % n)
+        status = np.zeros(max(1, n), dtype=np.int32)
+        tot = i64(0)
+        fn = self.lib.tb2_batch_alt_llr_motif
+        fn.restype = C.c_int
+        self.check(fn(self.handle, ptr(read_start, i64), ptr(strand, C.c_int8), C.byref(motif),
+                      i64(int(max_motif_bb)), i64(int(max_motif_ab)), i64(int(reg_start)),
+                      i64(int(reg_end)), C.c_int(int(bool(use_standard_llhr))),
+                      f64(scale_factor), f64(height_factor), f64(height_power),
+                      ptr(status, C.c_int32), C.byref(tot)))
+        self._llr_total, self._llr_reads = int(tot.value), read_start.shape[0]
+        return self._llr_total, status[:read_start.shape[0]].copy()
+
     def batch_llr_download(self):
         llr = np.empty(max(1, self._llr_total))
         pos = np.empty(max(1, self._llr_total), dtype=np.int64)
@@ -728,6 +801,19 @@ def make_policy(kind='DNA', outlier_thresh=5.0, max_raw_cpts=200,
                   int(kind == 'RNA'), int(bool(skip_seq_scaling)),
                   float('nan') if const_scale is None else const_scale,
                   subsample_seed, int(bool(rescue)))
+
+
+def ensure_model(ctx, std_ref):
+    """set ``std_ref`` (a TomboModel) as the context's canonical model, uploading the k-mer
+    tables once per model object.  The context keeps a strong reference (an id() alone can
+    be recycled after garbage collection) and a digest of the tables, so a model mutated in
+    place is uploaded again.  Every Python entry point that sets a model on a shared
+    context goes through here, so none of them can leave another one's cached model stale."""
+    m, s = std_ref.tables()
+    digest = hash((m.tobytes(), s.tobytes(), std_ref.kmer_width, std_ref.central_pos))
+    if getattr(ctx, '_model_ref', None) is not std_ref or getattr(ctx, '_model_digest', None) != digest:
+        ctx.set_model(m, s, std_ref.kmer_width, std_ref.central_pos)
+        ctx._model_ref, ctx._model_digest = std_ref, digest
 
 
 _default_ctx = {}

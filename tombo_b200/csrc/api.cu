@@ -132,6 +132,7 @@ extern "C" const char *tb2_status_message(int s)
     case TB2_ERR_SEG_COUNT: return "Aligned sequence does not match number of segments produced";
     case TB2_ERR_THEIL_SEN_ZERO: return "Read failed sequence-based signal re-scaling parameter estimation.";
     case TB2_ERR_INVALID_START_PATH: return "Invalid path through read start";
+    case TB2_ERR_READ_TOO_SHORT_IN_REGION: return "Read sequence too short in this region.";
     case TB2_ERR_UNEXPECTED: return "UNEXPECTED";
     case TB2_ERR_CUDA: return "CUDA error";
     case TB2_ERR_INVALID_ARG: return "invalid argument";

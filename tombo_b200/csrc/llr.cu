@@ -1,15 +1,20 @@
 // llr.cu -- per-read alternative-model log-likelihood ratios:
-// compute_alt_model_read_stats tombo_stats.py:3972-4082 (whole read, '+' strand,
-// single-base motif TomboMotif(alt_base, 1)) with trim_seq_and_means (:3888-3970),
-// c_calc_scaled_llh_ratio_const_var _c_helper.pyx:313-358 (default) and
-// c_calc_llh_ratio_const_var :298-311.  Also c_new_mean_stds :38-57.
+// compute_alt_model_read_stats tombo_stats.py:3972-4082 with trim_seq_and_means
+// (:3888-3970), c_calc_scaled_llh_ratio_const_var _c_helper.pyx:313-358 (default) and
+// c_calc_llh_ratio_const_var :298-311.  tb2_alt_model_llr_batch / tb2_batch_alt_llr score
+// whole '+' strand reads with a single-base motif TomboMotif(alt_base, 1);
+// tb2_alt_model_llr_motif_batch / tb2_batch_alt_llr_motif take any motif, both strands and
+// a region (the kernels are in motif_llr.cuh).  Also c_new_mean_stds :38-57.
 #include "batch.h"
+#include "motif_llr.cuh"
+#include <climits>
+#include <cstring>
 #include <vector>
 
 namespace {
 // per-call scratch of the entry points below; nothing reads it after a call returns
 enum { L_MEAN = 0, L_MOFF, L_SEQ, L_SOFF, L_START, L_CNT, L_SITEOFF, L_LLR, L_POS, L_A, L_B, L_C, L_D,
-       L_COUNT };
+       L_STRAND, L_STATUS, L_COUNT };
 }  // namespace
 
 struct LlrState {
@@ -22,24 +27,6 @@ struct LlrState {
 };
 
 namespace {
-struct LlrArgs {
-    int n_reads, K, cpos, alt_code, use_std;
-    double sf, hf, hp;
-    const double *norm_mean;
-    const long long *mean_off, *seq_off, *read_start;
-    const unsigned char *seq;
-    const double *kmeans, *ksds, *alt;   // alt[code * K + pos]
-    const int *status;                   // resident batch: reads that failed hold no sites
-    int status_stride;
-};
-
-__device__ __forceinline__ int kmer_code(const unsigned char *bases, int K)
-{
-    int c = 0;
-    for (int j = 0; j < K; ++j) c = c * 4 + (bases[j] & 3);
-    return c;
-}
-
 // FILL = false: count sites per read; FILL = true: write llr / pos
 template <bool FILL>
 __global__ void __launch_bounds__(256)
@@ -76,30 +63,7 @@ k_llr(LlrArgs a, int *counts, const long long *site_off, double *llr_out, long l
     for (int i = i0; i < i1; ++i) {
         if (bases[i + K - 1] != a.alt_code) continue;
         // alt_pos = i: k-mers i .. i+K-1 of the trimmed sequence, means' = means[cpos + .]
-        const double const_var = a.ksds[kmer_code(bases + i, K)];
-        const double cv = const_var * const_var;                 // np.square(r_ref_sds)[alt_pos]
-        double acc = 0.0;
-        for (int t = 0; t < K; ++t) {
-            const int code = kmer_code(bases + i + t, K);
-            const double obs = means[a.cpos + i + t];
-            const double ref_mean = a.kmeans[code];
-            const double alt_mean = a.alt[(size_t)code * K + (K - 1 - t)];
-            if (a.use_std) {
-                const double rd = obs - ref_mean, ad = obs - alt_mean;
-                acc += ((ad * ad) - (rd * rd)) / cv;
-            } else {
-                if (ref_mean == alt_mean) continue;
-                const double scale_mean = (alt_mean + ref_mean) / 2;
-                const double ref_diff = obs - ref_mean, alt_diff = obs - alt_mean;
-                const double scale_diff = obs - scale_mean;
-                double means_diff = alt_mean - ref_mean;
-                if (means_diff < 0) means_diff = means_diff * -1;
-                acc += exp(-(scale_diff * scale_diff) / (a.sf * cv)) *
-                       ((alt_diff * alt_diff) - (ref_diff * ref_diff)) /
-                       (cv * pow(means_diff, a.hp) * a.hf);
-            }
-        }
-        llr_out[o] = acc;
+        llr_out[o] = llr_site(a, bases, means, i);
         pos_out[o] = a.read_start[r] + (K - 1) + i;
         ++o;
     }
@@ -284,6 +248,182 @@ extern "C" int tb2_batch_alt_llr(tb2_ctx *ctx, const int64_t *read_start, int al
     TB2_CHECK_LAUNCH(ctx);
     long long total = 0;
     TB2_CUDA_TRY(ctx, cudaMemcpyAsync(&total, L.site_off.as<long long>() + n, 8, cudaMemcpyDeviceToHost, s));
+    TB2_CUDA_TRY(ctx, cudaStreamSynchronize(s));
+    L.sites = total;
+    L.reads = n;
+    if (n_sites_total) *n_sites_total = total;
+    return TB2_OK;
+}
+
+// ---------------------------------------------------------------------------
+// motif models, both strands, region clipping (k_llr_motif, motif_llr.cuh)
+// ---------------------------------------------------------------------------
+namespace {
+// checks shared by both motif entry points; fills everything of `a` but the read arrays
+int motif_args(tb2_ctx *ctx, const tb2_motif *motif, int64_t max_motif_bb, int64_t max_motif_ab,
+               int64_t reg_start, int64_t reg_end, int use_standard_llhr, double sf, double hf,
+               double hp, MotifArgs *a)
+{
+    if (!motif || motif->len < 1 || motif->len > 32 || motif->mod_pos < 1 ||
+        motif->mod_pos > motif->len)
+        return TB2_ERR_INVALID_ARG;
+    for (int j = 0; j < motif->len; ++j)
+        if (motif->mask[j] == 0 || motif->mask[j] > 15) return TB2_ERR_INVALID_ARG;
+    if (max_motif_bb < motif->mod_pos - 1 || max_motif_ab < motif->len - motif->mod_pos)
+        return TB2_ERR_INVALID_ARG;
+    if (ctx->kmer_width <= 0 || ctx->alt_kmer_width != ctx->kmer_width) {
+        ctx->err = "standard and alternative models must be set with the same k-mer width";
+        return TB2_ERR_INVALID_ARG;
+    }
+    memset(a, 0, sizeof(*a));
+    a->m.len = motif->len;
+    a->m.mod_pos = motif->mod_pos;
+    for (int j = 0; j < motif->len; ++j) a->m.mask[j] = motif->mask[j];
+    a->m.overlap = motif_can_overlap(a->m.mask, a->m.len) ? 1 : 0;
+    a->max_ab = max_motif_ab;
+    a->reg_start = reg_start;
+    a->reg_end = reg_end;
+    LlrArgs &s = a->s;
+    s.K = ctx->kmer_width; s.cpos = ctx->central_pos; s.alt_code = -1;
+    s.use_std = use_standard_llhr ? 1 : 0;
+    s.sf = sf; s.hf = hf; s.hp = hp;
+    s.kmeans = ctx->model_means.as<double>();
+    s.ksds = ctx->model_sds.as<double>();
+    s.alt = ctx->alt_means.as<double>();
+    return TB2_OK;
+}
+
+bool strands_ok(const int8_t *strand, int n)
+{
+    for (int r = 0; r < n; ++r)
+        if (strand[r] < -1 || strand[r] > 1) return false;
+    return true;
+}
+}  // namespace
+
+extern "C" int tb2_alt_model_llr_motif_batch(
+    tb2_ctx *ctx, int64_t n_reads, const double *norm_mean, const int64_t *mean_off,
+    const uint8_t *seq, const int64_t *seq_off, const int64_t *read_start, const int8_t *strand,
+    const tb2_motif *motif, int64_t max_motif_bb, int64_t max_motif_ab, int64_t reg_start,
+    int64_t reg_end, int use_standard_llhr, double scale_factor, double height_factor,
+    double height_power, double *llr_out, int64_t *pos_out, int64_t *site_off, int32_t *read_status)
+{
+    int rc = tb2_use(ctx);
+    if (rc) return rc;
+    if (n_reads < 0 || n_reads > INT_MAX || !mean_off || !seq_off || !read_start || !strand ||
+        !site_off)
+        return TB2_ERR_INVALID_ARG;
+    MotifArgs a;
+    if ((rc = motif_args(ctx, motif, max_motif_bb, max_motif_ab, reg_start, reg_end,
+                         use_standard_llhr, scale_factor, height_factor, height_power, &a)))
+        return rc;
+    const int n = (int)n_reads;
+    if (!strands_ok(strand, n)) return TB2_ERR_INVALID_ARG;
+    site_off[0] = 0;
+    if (n == 0) return TB2_OK;
+    if (!norm_mean || !seq || !llr_out || !pos_out) return TB2_ERR_INVALID_ARG;
+    // every read holds nb means and the nb + K - 1 bases of their k-mers
+    for (int r = 0; r < n; ++r) {
+        const long long nb = mean_off[r + 1] - mean_off[r];
+        if (nb < 0 || nb > INT_MAX || seq_off[r + 1] - seq_off[r] != nb + (ctx->kmer_width - 1))
+            return TB2_ERR_INVALID_ARG;
+    }
+    auto &P = tb2_state(ctx->llr).scratch;
+    cudaStream_t s = ctx->stream;
+    const size_t tm = (size_t)mean_off[n], ts = (size_t)seq_off[n];
+    TB2_CUDA_TRY(ctx, P[L_MEAN].reserve(tm * 8 + 8));
+    TB2_CUDA_TRY(ctx, P[L_MOFF].reserve((n + 1) * 8));
+    TB2_CUDA_TRY(ctx, P[L_SEQ].reserve(ts + 8));
+    TB2_CUDA_TRY(ctx, P[L_SOFF].reserve((n + 1) * 8));
+    TB2_CUDA_TRY(ctx, P[L_START].reserve((size_t)n * 8));
+    TB2_CUDA_TRY(ctx, P[L_STRAND].reserve((size_t)n));
+    TB2_CUDA_TRY(ctx, P[L_STATUS].reserve((size_t)n * 4));
+    TB2_CUDA_TRY(ctx, P[L_CNT].reserve((size_t)n * 4));
+    TB2_CUDA_TRY(ctx, P[L_SITEOFF].reserve((n + 1) * 8));
+    // every site is a base of its read: the mean count bounds the site count
+    TB2_CUDA_TRY(ctx, P[L_LLR].reserve(tm * 8 + 8));
+    TB2_CUDA_TRY(ctx, P[L_POS].reserve(tm * 8 + 8));
+    TB2_CUDA_TRY(ctx, cudaMemcpyAsync(P[L_MEAN].p, norm_mean, tm * 8, cudaMemcpyHostToDevice, s));
+    TB2_CUDA_TRY(ctx, cudaMemcpyAsync(P[L_MOFF].p, mean_off, (n + 1) * 8, cudaMemcpyHostToDevice, s));
+    TB2_CUDA_TRY(ctx, cudaMemcpyAsync(P[L_SEQ].p, seq, ts, cudaMemcpyHostToDevice, s));
+    TB2_CUDA_TRY(ctx, cudaMemcpyAsync(P[L_SOFF].p, seq_off, (n + 1) * 8, cudaMemcpyHostToDevice, s));
+    TB2_CUDA_TRY(ctx, cudaMemcpyAsync(P[L_START].p, read_start, (size_t)n * 8, cudaMemcpyHostToDevice, s));
+    TB2_CUDA_TRY(ctx, cudaMemcpyAsync(P[L_STRAND].p, strand, (size_t)n, cudaMemcpyHostToDevice, s));
+    a.s.n_reads = n;
+    a.s.norm_mean = P[L_MEAN].as<double>();
+    a.s.mean_off = P[L_MOFF].as<long long>();
+    a.s.seq_off = P[L_SOFF].as<long long>();
+    a.s.read_start = P[L_START].as<long long>();
+    a.s.seq = P[L_SEQ].as<unsigned char>();
+    a.strand = P[L_STRAND].as<signed char>();
+    a.read_status = P[L_STATUS].as<int>();
+    long long *d_off = P[L_SITEOFF].as<long long>();
+    k_llr_motif<false><<<n, 256, 0, s>>>(a, P[L_CNT].as<int>(), nullptr, nullptr, nullptr);
+    TB2_CHECK_LAUNCH(ctx);
+    k_scan_sites<<<1, 1024, 0, s>>>(P[L_CNT].as<int>(), d_off, n);
+    TB2_CHECK_LAUNCH(ctx);
+    k_llr_motif<true><<<n, 256, 0, s>>>(a, nullptr, d_off, P[L_LLR].as<double>(), P[L_POS].as<long long>());
+    TB2_CHECK_LAUNCH(ctx);
+    TB2_CUDA_TRY(ctx, cudaMemcpyAsync(site_off, d_off, (size_t)(n + 1) * 8, cudaMemcpyDeviceToHost, s));
+    if (read_status)
+        TB2_CUDA_TRY(ctx, cudaMemcpyAsync(read_status, P[L_STATUS].p, (size_t)n * 4, cudaMemcpyDeviceToHost, s));
+    TB2_CUDA_TRY(ctx, cudaStreamSynchronize(s));
+    const size_t total = (size_t)site_off[n];
+    if (total == 0) return TB2_OK;
+    TB2_CUDA_TRY(ctx, cudaMemcpyAsync(llr_out, P[L_LLR].p, total * 8, cudaMemcpyDeviceToHost, s));
+    TB2_CUDA_TRY(ctx, cudaMemcpyAsync(pos_out, P[L_POS].p, total * 8, cudaMemcpyDeviceToHost, s));
+    TB2_CUDA_TRY(ctx, cudaStreamSynchronize(s));
+    return TB2_OK;
+}
+
+extern "C" int tb2_batch_alt_llr_motif(tb2_ctx *ctx, const int64_t *read_start, const int8_t *strand,
+                                       const tb2_motif *motif, int64_t max_motif_bb,
+                                       int64_t max_motif_ab, int64_t reg_start, int64_t reg_end,
+                                       int use_standard_llhr, double scale_factor,
+                                       double height_factor, double height_power,
+                                       int32_t *read_status, int64_t *n_sites_total)
+{
+    int rc = tb2_use(ctx);
+    if (rc) return rc;
+    if (!read_start || !strand) return TB2_ERR_INVALID_ARG;
+    MotifArgs a;
+    if ((rc = motif_args(ctx, motif, max_motif_bb, max_motif_ab, reg_start, reg_end,
+                         use_standard_llhr, scale_factor, height_factor, height_power, &a)))
+        return rc;
+    BatchResultView v;
+    if ((rc = tb2_batch_result_view(ctx, &v))) return rc;
+    const int n = v.n_reads;
+    if (!strands_ok(strand, n)) return TB2_ERR_INVALID_ARG;
+    LlrState &L = tb2_state(ctx->llr);
+    auto &P = L.scratch;
+    cudaStream_t s = ctx->stream;
+    TB2_CUDA_TRY(ctx, P[L_START].reserve((size_t)n * 8));
+    TB2_CUDA_TRY(ctx, P[L_STRAND].reserve((size_t)n));
+    TB2_CUDA_TRY(ctx, P[L_STATUS].reserve((size_t)n * 4));
+    TB2_CUDA_TRY(ctx, P[L_CNT].reserve((size_t)n * 4));
+    TB2_CUDA_TRY(ctx, L.site_off.reserve((size_t)(n + 1) * 8));
+    TB2_CUDA_TRY(ctx, L.llr.reserve((size_t)v.total_bases * 8 + 8));
+    TB2_CUDA_TRY(ctx, L.pos.reserve((size_t)v.total_bases * 8 + 8));
+    TB2_CUDA_TRY(ctx, cudaMemcpyAsync(P[L_START].p, read_start, (size_t)n * 8, cudaMemcpyHostToDevice, s));
+    TB2_CUDA_TRY(ctx, cudaMemcpyAsync(P[L_STRAND].p, strand, (size_t)n, cudaMemcpyHostToDevice, s));
+    a.s.n_reads = n;
+    a.s.norm_mean = v.norm_mean; a.s.mean_off = v.base_off; a.s.seq_off = v.seq_off;
+    a.s.read_start = P[L_START].as<long long>();
+    a.s.seq = v.seq;
+    a.s.status = v.status; a.s.status_stride = v.stride;
+    a.strand = P[L_STRAND].as<signed char>();
+    a.read_status = P[L_STATUS].as<int>();
+    k_llr_motif<false><<<n, 256, 0, s>>>(a, P[L_CNT].as<int>(), nullptr, nullptr, nullptr);
+    TB2_CHECK_LAUNCH(ctx);
+    k_scan_sites<<<1, 1024, 0, s>>>(P[L_CNT].as<int>(), L.site_off.as<long long>(), n);
+    TB2_CHECK_LAUNCH(ctx);
+    k_llr_motif<true><<<n, 256, 0, s>>>(a, nullptr, L.site_off.as<long long>(), L.llr.as<double>(),
+                                        L.pos.as<long long>());
+    TB2_CHECK_LAUNCH(ctx);
+    long long total = 0;
+    TB2_CUDA_TRY(ctx, cudaMemcpyAsync(&total, L.site_off.as<long long>() + n, 8, cudaMemcpyDeviceToHost, s));
+    if (read_status)
+        TB2_CUDA_TRY(ctx, cudaMemcpyAsync(read_status, P[L_STATUS].p, (size_t)n * 4, cudaMemcpyDeviceToHost, s));
     TB2_CUDA_TRY(ctx, cudaStreamSynchronize(s));
     L.sites = total;
     L.reads = n;

@@ -34,14 +34,8 @@ def _seq_codes(seq):
 
 
 def _ensure_model(ctx, std_ref):
-    """upload the k-mer tables once per model object.  The context keeps a strong
-    reference (an id() alone can be recycled after garbage collection) and a digest of
-    the tables, so a model mutated in place is uploaded again."""
-    m, s = std_ref.tables()
-    digest = hash((m.tobytes(), s.tobytes(), std_ref.kmer_width, std_ref.central_pos))
-    if getattr(ctx, '_model_ref', None) is not std_ref or getattr(ctx, '_model_digest', None) != digest:
-        ctx.set_model(m, s, std_ref.kmer_width, std_ref.central_pos)
-        ctx._model_ref, ctx._model_digest = std_ref, digest
+    """upload the k-mer tables once per model object (_lib.ensure_model)"""
+    _lib.ensure_model(ctx, std_ref)
 
 
 # ---------------------------------------------------------------------------

@@ -19,7 +19,7 @@ __all__ = [
     'TomboModel', 'AltModel', 'normalize_raw_signal', 'compute_base_means',
     'get_read_seg_score', 'calc_kmer_fitted_shift_scale', 'load_resquiggle_parameters',
     'compute_num_events', 'get_dynamic_prog_params', 'identify_stalls',
-    'compute_alt_model_read_stats', 'trim_seq_and_means', 'apply_per_read_thresh',
+    'compute_alt_model_read_stats', 'compute_alt_model_reads_stats', 'trim_seq_and_means', 'apply_per_read_thresh',
     'collate_reg_stats', 'calc_damp_fraction', 'calc_window_fishers_method',
     'compute_de_novo_read_stats', 'compute_sample_compare_read_stats',
     'compute_ks_tests', 'compute_u_tests', 'compute_t_tests', 'calc_window_means',
@@ -397,6 +397,94 @@ def compute_alt_model_read_stats(r_data, std_ref, alt_refs, use_standard_llhr=Fa
         all_llhrs[alt_name] = llhrs
         all_poss[alt_name] = gen_poss
     return all_llhrs, all_poss, read_id
+
+
+_BASE_CODE = np.full(256, 255, dtype=np.uint8)
+_BASE_CODE[np.frombuffer(b'ACGT', dtype=np.uint8)] = np.arange(4, dtype=np.uint8)
+
+
+def compute_alt_model_reads_stats(r_datas, std_ref, alt_refs, use_standard_llhr=False,
+                                  reg_data=None, device=0):
+    """Batched :func:`compute_alt_model_read_stats`: every read of ``r_datas`` (either strand)
+    against every alt model of ``alt_refs`` (any ``TomboMotif``), clipped to ``reg_data``
+    (None: whole reads), in one device call per alt model.  Read data arrive through the same
+    FAST5 seam.  Returns, per read, ``(all_llhrs, all_poss, read_id)`` or the
+    :class:`tombo_helper.TomboError` the reference would raise for that read.
+
+    Two whole-read checks run before the region clip, where the reference would first clip
+    and then look up levels: a read with a non-ACGT base anywhere fails with 'Invalid
+    sequence encountered from genome sequence.' even if the region would clip that base
+    away, and a read whose base and level counts differ fails with 'Mismatching k-mer and
+    mean levels.' before it could be found too short.  Non-ACGT reference bases are outside
+    what the device batch accepts; resquiggled reads always carry one level per base."""
+    K, cpos = std_ref.kmer_width, std_ref.central_pos
+    max_motif_bb = max([alt_ref.motif.mod_pos - 1 for _, alt_ref in alt_refs])
+    max_motif_ab = max([alt_ref.motif.motif_len - alt_ref.motif.mod_pos
+                        for _, alt_ref in alt_refs])
+    out = [None] * len(r_datas)
+    means, codes, starts, strands, ids, idx = [], [], [], [], [], []
+    for i, r_data in enumerate(r_datas):
+        r_means, r_seq = th.get_multiple_slots_read_centric(
+            r_data, ['norm_mean', 'base'], r_data.corr_group)
+        try:
+            read_id = th.get_raw_read_slot(r_data).attrs.get('read_id')
+        except Exception:
+            read_id = getattr(r_data, 'read_id', None)
+        if r_means is None or r_seq is None:
+            out[i] = th.TomboError('Read does not contain valid re-squiggled data.')
+            continue
+        r_seq = b''.join(r_seq) if not isinstance(r_seq, str) else r_seq.encode()
+        c = _BASE_CODE[np.frombuffer(r_seq, dtype=np.uint8)]
+        if (c > 3).any():
+            # non-ACGT bases: the reference fails the k-mer level look-up
+            out[i] = th.TomboError('Invalid sequence encountered from genome sequence.')
+            continue
+        r_means = np.asarray(r_means, dtype=np.float64)
+        if c.shape[0] != r_means.shape[0]:
+            out[i] = th.TomboError('Mismatching k-mer and mean levels.')
+            continue
+        # the library's layout: nb + K - 1 codes, the read's bases cpos codes in
+        means.append(r_means)
+        codes.append(np.concatenate([np.zeros(cpos, np.uint8), c,
+                                     np.zeros(K - 1 - cpos, np.uint8)]))
+        starts.append(r_data.start)
+        strands.append(0 if r_data.strand == '+' else 1)
+        ids.append(read_id)
+        idx.append(i)
+    if not idx:
+        return out
+    nbs = np.array([m.shape[0] for m in means], dtype=np.int64)
+    starts = np.array(starts, dtype=np.int64)
+    if reg_data is not None:
+        reg_start, reg_end = reg_data.start, reg_data.end
+    else:
+        # a region that contains every read leaves each one whole
+        reg_start, reg_end = int(starts.min()), int((starts + nbs).max())
+    norm_mean = np.concatenate(means)
+    mean_off = np.concatenate([[0], np.cumsum(nbs)]).astype(np.int64)
+    seq = np.concatenate(codes)
+    seq_off = np.concatenate([[0], np.cumsum(nbs + K - 1)]).astype(np.int64)
+    strands = np.array(strands, dtype=np.int8)
+    ctx = _lib.get_context(device)
+    _lib.ensure_model(ctx, std_ref)
+    per_read = [({}, {}) for _ in idx]
+    status = None
+    for alt_name, alt_ref in alt_refs:
+        ctx.set_alt_model(alt_ref.table(), alt_ref.kmer_width)
+        llr, pos, off, status = ctx.alt_model_llr_motif_batch(
+            norm_mean, mean_off, seq, seq_off, starts, strands,
+            _lib.motif_struct(alt_ref.motif), max_motif_bb, max_motif_ab, reg_start, reg_end,
+            use_standard_llhr, OCLLHR_SCALE, OCLLHR_HEIGHT, OCLLHR_POWER)
+        for j in range(len(idx)):
+            a, b = int(off[j]), int(off[j + 1])
+            per_read[j][0][alt_name] = llr[a:b] if b > a else np.array([])
+            per_read[j][1][alt_name] = pos[a:b] if b > a else np.array([])
+    for j, i in enumerate(idx):
+        if status[j] != 0:
+            out[i] = th.TomboError(_lib.status_message(status[j]))
+        else:
+            out[i] = (per_read[j][0], per_read[j][1], ids[j])
+    return out
 
 
 # ---------------------------------------------------------------------------
