@@ -89,8 +89,6 @@ def test_pipeline_chunk_schedule_covers_every_read_once():
     from tombo_b200 import _lib
     lib = _lib.load()
     fn = lib.tb2_pipeline_chunks
-    fn.restype = ctypes.c_int
-    fn.argtypes = [ctypes.c_int, ctypes.c_int64, ctypes.POINTER(ctypes.c_int64), ctypes.c_int]
     buf = (ctypes.c_int64 * 4096)()
     sm = 132                              # H100 SXM
     unit = sm * 32
@@ -109,3 +107,64 @@ def test_pipeline_chunk_schedule_covers_every_read_once():
             assert k >= 2 and sizes[0] == 2 * unit   # short first chunk: its upload is exposed
     assert fn(sm, 10 ** 9, buf, 8) < 0        # capacity is reported, not overrun
     assert fn(sm, -1, buf, 8) < 0
+
+
+def header_prototypes():
+    """{name: (return spelling, [argument spellings])} of include/tombo_b200.h, each spelling
+    with single spaces and the '*'s joined to the type, e.g. 'const int64_t*'"""
+    src = open(os.path.join(REPO, 'include', 'tombo_b200.h')).read()
+    src = re.sub(r'/\*.*?\*/|//[^\n]*|#[^\n]*', ' ', src, flags=re.S)
+
+    def spelling(decl, named):
+        words = decl.replace('*', ' * ').split()
+        if named:
+            words = words[:-1]                      # the parameter name
+        return ' '.join(words).replace(' *', '*')
+    protos = {}
+    for ret, name, args in re.findall(r'([A-Za-z_][\w\s*]*?)\b(tb2_\w+)\s*\(([^)]*)\)\s*;', src):
+        args = [] if args.strip() in ('', 'void') else args.split(',')
+        protos[name] = (spelling(ret, False), [spelling(a, True) for a in args])
+    return protos
+
+
+def ctype_of(spelling):
+    """the ctypes type the binding must use for one C type spelling of the header"""
+    from tombo_b200 import _lib
+    scalars = {'void': None, 'int': ctypes.c_int, 'int8_t': ctypes.c_int8,
+               'uint8_t': ctypes.c_uint8, 'int32_t': ctypes.c_int32, 'int64_t': ctypes.c_int64,
+               'uint32_t': ctypes.c_uint32, 'uint64_t': ctypes.c_uint64,
+               'unsigned long long': ctypes.c_ulonglong, 'size_t': ctypes.c_size_t,
+               'double': ctypes.c_double, 'tb2_params': _lib.Params, 'tb2_policy': _lib.Policy,
+               'tb2_scale_values': _lib.ScaleValues, 'tb2_motif': _lib.Motif}
+    t = spelling.replace('const ', '')
+    if t in ('void*', 'tb2_ctx*'):                  # tb2_ctx is opaque: a handle
+        return ctypes.c_void_p
+    if t == 'char*':
+        return ctypes.c_char_p
+    if t.endswith('*'):
+        return ctypes.POINTER(ctype_of(t[:-1]))
+    return scalars[t]
+
+
+def test_binding_prototypes_match_header():
+    """_lib._PROTOS types every function of the header, and only those (no .so needed)"""
+    from tombo_b200 import _lib
+    protos = header_prototypes()
+    assert len(protos) >= 50
+    assert sorted(_lib._PROTOS) == sorted(protos)
+    for name, (ret, args) in protos.items():
+        res, argtypes = _lib._PROTOS[name]
+        assert res is ctype_of(ret), (name, ret, res)
+        assert len(argtypes) == len(args), (name, len(argtypes), len(args))
+        for i, (a, t) in enumerate(zip(args, argtypes)):
+            assert t is ctype_of(a), (name, i, a, t)
+
+
+def test_package_calls_only_declared_functions():
+    import glob
+    protos = header_prototypes()
+    used = set()
+    for path in glob.glob(os.path.join(REPO, 'tombo_b200', '*.py')):
+        used |= set(re.findall(r'\.(tb2_\w+)\b', open(path).read()))
+    assert used, 'no library calls found'
+    assert not used - set(protos), sorted(used - set(protos))

@@ -9,7 +9,6 @@ pytestmark = pytest.mark.gpu
 
 def test_div_by_reciprocal_is_correctly_rounded(ctx):
     fn = ctx.lib.tb2_debug_div_check
-    fn.restype = C.c_int
     total = 0
     for seed in (1, 2, 3, 4):
         mism = C.c_uint64(0)

@@ -115,6 +115,37 @@ def test_llr_batch_rejects_a_sequence_longer_than_its_means(ctx):
         ctx.alt_model_llr_batch(nm, mo, sq_long, so_long, np.zeros(3, np.int64), 1)
 
 
+@pytest.mark.parametrize('call', ['llr', 'motif', 'de_novo'])
+def test_host_array_calls_reject_counts_past_int_max(ctx, call):
+    """the kernels index reads and bases with int: 2^31 reads, or one read of 2^31 bases, is an
+    invalid argument, found before any array is read past its first entries (the arrays here
+    hold two)"""
+    from tombo_b200 import _lib
+    K, cpos, means, sds, alt = _tables('dna6')
+    ctx.set_model(means, sds, K, cpos)
+    ctx.set_alt_model(alt, K)
+    p64, pf = (lambda a: _lib.ptr(a, _lib.i64)), (lambda a: _lib.ptr(a, _lib.f64))
+    nm, llr, start = np.zeros(2), np.zeros(2), np.zeros(2, np.int64)
+    pos, site_off = np.zeros(2, np.int64), np.zeros(2, np.int64)
+    sq, strand, status = np.zeros(2, np.uint8), np.zeros(2, np.int8), np.zeros(2, np.int32)
+    motif = _lib.Motif(1, 1)
+    motif.mask[0] = 2
+    big = 2 ** 31
+    for n_reads, mo, so in ((big, np.zeros(2, np.int64), np.zeros(2, np.int64)),
+                            (1, np.array([0, big], np.int64), np.array([0, big + K - 1], np.int64))):
+        head = (ctx.handle, n_reads, pf(nm), p64(mo), _lib.ptr(sq, C.c_uint8), p64(so), p64(start))
+        if call == 'llr':
+            rc = ctx.lib.tb2_alt_model_llr_batch(*head, 1, 0, 4.0, 1.0, 0.2, pf(llr), p64(pos),
+                                                 p64(site_off))
+        elif call == 'motif':
+            rc = ctx.lib.tb2_alt_model_llr_motif_batch(
+                *head, _lib.ptr(strand, C.c_int8), C.byref(motif), 0, 0, 0, 10 ** 6, 0, 4.0, 1.0,
+                0.2, pf(llr), p64(pos), p64(site_off), _lib.ptr(status, C.c_int32))
+        else:
+            rc = ctx.lib.tb2_de_novo_read_stats_batch(*head, 1, pf(llr), p64(pos), p64(site_off))
+        assert rc == 201, (call, n_reads, rc)                # TB2_ERR_INVALID_ARG
+
+
 # ---------------------------------------------------------------------------
 # tb2_batch_alt_llr on a resident batch of >= 2 500 reads (three k_scan_sites chunks)
 # ---------------------------------------------------------------------------
@@ -402,12 +433,11 @@ def test_region_finalize_reports_capacity(ctx):
                damp_frac=np.full(cap, -1.0), cov=np.full(cap, -1, np.int64),
                valid_cov=np.full(cap, -1, np.int64))
     n = C.c_int64(0)
-    fn = ctx.lib.tb2_region_stats_finalize
-    fn.restype = C.c_int
-    rc = fn(ctx.handle, C.c_double(2.0), C.c_double(0.0), C.c_int64(cap),
-            _lib.ptr(out['pos'], _lib.i64), _lib.ptr(out['frac'], _lib.f64),
-            _lib.ptr(out['damp_frac'], _lib.f64), _lib.ptr(out['cov'], _lib.i64),
-            _lib.ptr(out['valid_cov'], _lib.i64), C.byref(n))
+    rc = ctx.lib.tb2_region_stats_finalize(
+        ctx.handle, C.c_double(2.0), C.c_double(0.0), C.c_int64(cap),
+        _lib.ptr(out['pos'], _lib.i64), _lib.ptr(out['frac'], _lib.f64),
+        _lib.ptr(out['damp_frac'], _lib.f64), _lib.ptr(out['cov'], _lib.i64),
+        _lib.ptr(out['valid_cov'], _lib.i64), C.byref(n))
     assert rc == 202                                     # TB2_ERR_CAPACITY
     assert n.value == n_cov
     for k in out:

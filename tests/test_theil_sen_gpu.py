@@ -19,9 +19,7 @@ BY_NAME = {c.name: c for c in CASES}
 def debug_counters(ctx):
     """g_tb2_counters (include/tombo_b200.h); device-global, so callers compare deltas"""
     out = (C.c_ulonglong * 8)()
-    fn = ctx.lib.tb2_debug_counters
-    fn.restype = C.c_int
-    ctx.check(fn(ctx.handle, out, 0))
+    ctx.check(ctx.lib.tb2_debug_counters(ctx.handle, out, 0))
     return np.array(list(out), dtype=np.int64)
 
 

@@ -69,15 +69,77 @@ def motif_struct(motif):
 _lib = None
 _lock = threading.Lock()
 
+# (return type, argument types) of every function in include/tombo_b200.h, in its order; tb2_ctx * is
+# an opaque handle.  tests/test_abi_cpu.py checks this table against the header.
+_I, _CTX = C.c_int, C.c_void_p
+pI, pI32, pI64, pF64 = P(C.c_int), P(C.c_int32), P(i64), P(f64)
+pI8, pU8 = P(C.c_int8), P(C.c_uint8)
+pPar, pPol, pSV, pMotif = P(Params), P(Policy), P(ScaleValues), P(Motif)
 _PROTOS = {
-    'tb2_abi_version': (C.c_int, []),
-    'tb2_device_count': (C.c_int, []),
-    'tb2_ctx_create': (C.c_int, [C.c_int, P(C.c_void_p)]),
-    'tb2_ctx_destroy': (None, [C.c_void_p]),
-    'tb2_status_message': (C.c_char_p, [C.c_int]),
-    'tb2_last_error': (C.c_char_p, [C.c_void_p]),
-    'tb2_launch_count': (i64, [C.c_void_p]),
-    'tb2_last_timing': (C.c_int, [C.c_void_p, P(f64)]),
+    'tb2_abi_version': (_I, []),
+    'tb2_device_count': (_I, []),
+    'tb2_ctx_create': (_I, [_I, P(_CTX)]),
+    'tb2_ctx_destroy': (None, [_CTX]),
+    'tb2_status_message': (C.c_char_p, [_I]),
+    'tb2_last_error': (C.c_char_p, [_CTX]),
+    'tb2_launch_count': (i64, [_CTX]),
+    'tb2_last_timing': (_I, [_CTX, pF64]),
+    'tb2_host_alloc': (C.c_void_p, [C.c_size_t]),
+    'tb2_host_free': (None, [C.c_void_p]),
+    'tb2_set_model': (_I, [_CTX, pF64, pF64, _I, _I]),
+    'tb2_set_alt_model': (_I, [_CTX, pF64, _I]),
+    'tb2_new_means': (_I, [_CTX, pF64, i64, pI64, i64, pF64]),
+    'tb2_new_mean_stds': (_I, [_CTX, pF64, i64, pI64, i64, pF64, pF64]),
+    'tb2_normalize_raw_signal': (_I, [_CTX, pF64, i64, _I, f64, f64, pSV, pF64, pSV]),
+    'tb2_identify_stalls': (_I, [_CTX, pF64, i64, pI64, i64, pI64]),
+    'tb2_valid_cpts_w_cap': (_I, [_CTX, pF64, i64, i64, i64, i64, _I, pI64, pI]),
+    'tb2_banded_forward_pass': (_I, [_CTX, pF64, pI64, i64, i64, f64, f64, pF64, pI64]),
+    'tb2_banded_traceback': (_I, [_CTX, pI64, pI64, i64, i64, i64, i64, pI64, pI]),
+    'tb2_adaptive_banded_forward_pass': (_I, [_CTX, pF64, pI64, pI64, i64, i64, pF64, i64, pF64,
+                                              pF64, f64, f64, f64, i64, f64, _I, f64, pI]),
+    'tb2_theil_sen': (_I, [_CTX, f64, f64, pF64, pF64, i64, C.c_uint32, pF64, pI]),
+    'tb2_find_adaptive_base_assignment': (_I, [_CTX, pI64, i64, pF64, pPar, pF64, pF64, i64, f64,
+                                               pI64, pI64, pI64, pI]),
+    'tb2_find_static_base_assignment': (_I, [_CTX, pF64, i64, pF64, pF64, i64, pPar, pI64, pI]),
+    'tb2_find_seq_start_in_events': (_I, [_CTX, pF64, i64, pF64, pF64, i64, pPar, i64, i64, _I,
+                                          f64, pI64, pF64, pI]),
+    'tb2_debug_div_check': (_I, [_CTX, C.c_uint64, _I, _I, P(C.c_uint64), pF64]),
+    'tb2_debug_counters': (_I, [_CTX, P(C.c_ulonglong), _I]),
+    'tb2_resolve_skipped_bases_with_raw': (_I, [_CTX, pI64, i64, pF64, pF64, pF64, i64, pPar, i64,
+                                                pI64, pI]),
+    'tb2_resquiggle_batch': (_I, [_CTX, i64, C.c_void_p, _I, pI64, pU8, pI64, pPar, pPar, pPol,
+                                  pI64, pI64, pSV, pF64, pF64, pF64, pI32, pI32, pI32]),
+    'tb2_pipeline_chunks': (_I, [_I, i64, pI64, _I]),
+    'tb2_batch_upload': (_I, [_CTX, i64, C.c_void_p, _I, pI64, pU8, pI64, pPar, pPol]),
+    'tb2_batch_set_read_inputs': (_I, [_CTX, pSV, pI64, pI64]),
+    'tb2_batch_compute': (_I, [_CTX, pPar, pPar, pPol, _I]),
+    'tb2_batch_download': (_I, [_CTX, pI64, pI64, pSV, pF64, pF64, pF64, pI32, pI32, pI32]),
+    'tb2_alt_model_llr_batch': (_I, [_CTX, i64, pF64, pI64, pU8, pI64, pI64, _I, _I, f64, f64, f64,
+                                     pF64, pI64, pI64]),
+    'tb2_calc_llh_ratio_windows': (_I, [_CTX, _I, i64, _I, pF64, pF64, pF64, pF64, pF64, f64, f64,
+                                        f64, pF64]),
+    'tb2_timer_start': (_I, [_CTX]),
+    'tb2_timer_stop': (_I, [_CTX, pF64]),
+    'tb2_batch_alt_llr': (_I, [_CTX, pI64, _I, _I, f64, f64, f64, pI64]),
+    'tb2_batch_llr_download': (_I, [_CTX, pF64, pI64, pI64]),
+    'tb2_alt_model_llr_motif_batch': (_I, [_CTX, i64, pF64, pI64, pU8, pI64, pI64, pI8, pMotif, i64,
+                                           i64, i64, i64, _I, f64, f64, f64, pF64, pI64, pI64,
+                                           pI32]),
+    'tb2_batch_alt_llr_motif': (_I, [_CTX, pI64, pI8, pMotif, i64, i64, i64, i64, _I, f64, f64, f64,
+                                     pI32, pI64]),
+    'tb2_region_stats_begin': (_I, [_CTX, i64, i64]),
+    'tb2_region_stats_add': (_I, [_CTX, i64, pF64, pI64, f64, f64, _I]),
+    'tb2_region_stats_add_batch_llr': (_I, [_CTX, f64, f64, _I]),
+    'tb2_region_counts_get': (_I, [_CTX, pI32]),
+    'tb2_region_counts_set': (_I, [_CTX, pI32]),
+    'tb2_region_stats_finalize': (_I, [_CTX, f64, f64, i64, pI64, pF64, pF64, pI64, pI64, pI64]),
+    'tb2_window_fisher_pvals': (_I, [_CTX, i64, pF64, pF64, pF64, pI64, i64, _I, pF64]),
+    'tb2_de_novo_read_stats_batch': (_I, [_CTX, i64, pF64, pI64, pU8, pI64, pI64, i64, pF64, pI64,
+                                          pI64]),
+    'tb2_group_reg_stats': (_I, [_CTX, i64, i64, i64, pF64, pI64, pI64, i64, pF64, pI64, pI64, _I,
+                                 _I, i64, i64, i64, pI64, pF64, pI64, pI64, pI64]),
+    'tb2_reads_ref_levels': (_I, [_CTX, i64, i64, i64, pF64, pI64, pI64, i64, _I, pF64, pF64, f64,
+                                  f64, pF64, pF64, pI64]),
 }
 
 
@@ -109,9 +171,6 @@ class PinnedArray(object):
 
     def __init__(self, shape, dtype):
         lib = load()
-        lib.tb2_host_alloc.restype = C.c_void_p
-        lib.tb2_host_alloc.argtypes = [C.c_size_t]
-        lib.tb2_host_free.argtypes = [C.c_void_p]
         self._lib = lib
         dt = np.dtype(dtype)
         n = int(np.prod(shape))
@@ -124,7 +183,7 @@ class PinnedArray(object):
     def free(self):
         if self._p:
             self.array = None
-            self._lib.tb2_host_free(C.c_void_p(self._p))
+            self._lib.tb2_host_free(self._p)
             self._p = None
 
 
@@ -138,6 +197,38 @@ def as_i64(a):
 
 def ptr(a, ctype):
     return a.ctypes.data_as(P(ctype))
+
+
+def _offsets(seq_off, k):
+    """base_off / seg_off of a batch: sequences shorter than the k-mer map zero bases (the
+    library clamps the same way), and each read has one more segment boundary than bases"""
+    nb = np.maximum((seq_off[1:] - seq_off[:-1]) - (k - 1), 0)
+    base_off = np.concatenate([[0], np.cumsum(nb)]).astype(np.int64)
+    return base_off, base_off + np.arange(base_off.shape[0], dtype=np.int64)
+
+
+def _batch_outputs(out, base_off, seg_off, n_samples, want_norm_signal):
+    """the nine output pointers of tb2_resquiggle_batch / tb2_batch_download, into arrays of
+    ``out`` that fit (new ones otherwise)"""
+    n = base_off.shape[0] - 1
+
+    def buf(name, shape, dt):
+        a = out.get(name)
+        if a is None or a.shape != tuple(np.atleast_1d(shape)) or a.dtype != dt:
+            a = out[name] = np.empty(shape, dtype=dt)
+        return a
+    segs = buf('segs', int(seg_off[-1]), np.int64)
+    rsrtr = buf('read_start_rel_to_raw', n, np.int64)
+    sv = buf('scale_values', (n, 5), np.float64)
+    score = buf('sig_match_score', n, np.float64)
+    norm_mean = buf('norm_mean', int(base_off[-1]), np.float64)
+    status = buf('status', n, np.int32)
+    n_iters = buf('n_iters', n, np.int32)
+    flags = buf('flags', n, np.int32)
+    norm_sig = buf('norm_signal', n_samples, np.float64) if want_norm_signal else None
+    return (ptr(segs, i64), ptr(rsrtr, i64), ptr(sv, ScaleValues), ptr(score, f64),
+            ptr(norm_mean, f64), ptr(norm_sig, f64) if norm_sig is not None else None,
+            ptr(status, C.c_int32), ptr(n_iters, C.c_int32), ptr(flags, C.c_int32))
 
 
 def params_struct(p):
@@ -194,16 +285,12 @@ class Context(object):
         return int(self.lib.tb2_launch_count(self.handle))
 
     def timer_start(self):
-        fn = self.lib.tb2_timer_start
-        fn.restype = C.c_int
-        self.check(fn(self.handle))
+        self.check(self.lib.tb2_timer_start(self.handle))
 
     def timer_stop(self):
         """device milliseconds since timer_start (CUDA events on the library's stream)"""
         ms = f64(0.0)
-        fn = self.lib.tb2_timer_stop
-        fn.restype = C.c_int
-        self.check(fn(self.handle, C.byref(ms)))
+        self.check(self.lib.tb2_timer_stop(self.handle, C.byref(ms)))
         return float(ms.value)
 
     def last_timing(self):
@@ -221,18 +308,11 @@ class Context(object):
         raw_off, seq_off = as_i64(raw_off), as_i64(seq_off)
         seq = np.ascontiguousarray(seq, dtype=np.uint8)
         p = params if isinstance(params, Params) else params_struct(params)
-        fn = self.lib.tb2_batch_upload
-        fn.restype = C.c_int
-        self.check(fn(self.handle, i64(raw_off.shape[0] - 1),
-                      raw.ctypes.data_as(C.c_void_p), C.c_int(dtype),
-                      ptr(raw_off, i64), ptr(seq, C.c_uint8), ptr(seq_off, i64),
-                      C.byref(p), C.byref(policy)))
-        k = self.kmer_width
-        n = raw_off.shape[0] - 1
-        # sequences shorter than the k-mer map zero bases (the library clamps the same way)
-        nb = np.maximum((seq_off[1:] - seq_off[:-1]) - (k - 1), 0)
-        self._base_off = np.concatenate([[0], np.cumsum(nb)]).astype(np.int64)
-        self._seg_off = self._base_off + np.arange(n + 1, dtype=np.int64)
+        self.check(self.lib.tb2_batch_upload(self.handle, raw_off.shape[0] - 1,
+                                             raw.ctypes.data_as(C.c_void_p), dtype,
+                                             ptr(raw_off, i64), ptr(seq, C.c_uint8),
+                                             ptr(seq_off, i64), C.byref(p), C.byref(policy)))
+        self._base_off, self._seg_off = _offsets(seq_off, self.kmer_width)
         self._n_samples = int(raw_off[-1])
 
     def batch_compute(self, params, save_params, policy, want_norm_signal=False):
@@ -240,38 +320,16 @@ class Context(object):
         sp = None
         if save_params is not None:
             sp = save_params if isinstance(save_params, Params) else params_struct(save_params)
-        fn = self.lib.tb2_batch_compute
-        fn.restype = C.c_int
-        self.check(fn(self.handle, C.byref(p), C.byref(sp) if sp is not None else None,
-                      C.byref(policy), C.c_int(int(bool(want_norm_signal)))))
+        self.check(self.lib.tb2_batch_compute(self.handle, C.byref(p),
+                                              C.byref(sp) if sp is not None else None,
+                                              C.byref(policy), int(bool(want_norm_signal))))
 
     def batch_download(self, want_norm_signal=False, out=None):
         base_off, seg_off = self._base_off, self._seg_off
-        n = base_off.shape[0] - 1
         if out is None:
             out = {}
-
-        def buf(name, shape, dt):
-            a = out.get(name)
-            if a is None or a.shape != tuple(np.atleast_1d(shape)) or a.dtype != dt:
-                a = out[name] = np.empty(shape, dtype=dt)
-            return a
-        segs = buf('segs', int(seg_off[-1]), np.int64)
-        rsrtr = buf('read_start_rel_to_raw', n, np.int64)
-        sv = buf('scale_values', (n, 5), np.float64)
-        score = buf('sig_match_score', n, np.float64)
-        norm_mean = buf('norm_mean', int(base_off[-1]), np.float64)
-        status = buf('status', n, np.int32)
-        n_iters = buf('n_iters', n, np.int32)
-        flags = buf('flags', n, np.int32)
-        norm_sig = buf('norm_signal', self._n_samples, np.float64) if want_norm_signal else None
-        fn = self.lib.tb2_batch_download
-        fn.restype = C.c_int
-        self.check(fn(self.handle, ptr(segs, i64), ptr(rsrtr, i64),
-                      sv.ctypes.data_as(C.c_void_p), ptr(score, f64), ptr(norm_mean, f64),
-                      ptr(norm_sig, f64) if norm_sig is not None else None,
-                      ptr(status, C.c_int32), ptr(n_iters, C.c_int32),
-                      ptr(flags, C.c_int32)))
+        outs = _batch_outputs(out, base_off, seg_off, self._n_samples, want_norm_signal)
+        self.check(self.lib.tb2_batch_download(self.handle, *outs))
         out['base_off'], out['seg_off'] = base_off, seg_off
         return out
 
@@ -282,10 +340,9 @@ class Context(object):
         nb, bw = z.shape
         fwd = np.empty((nb + 1, bw))
         tb = np.empty((nb + 1, bw), dtype=np.int64)
-        fn = self.lib.tb2_banded_forward_pass
-        fn.restype = C.c_int
-        self.check(fn(self.handle, ptr(z, f64), ptr(es, i64), i64(nb), i64(bw),
-                      f64(skip_pen), f64(stay_pen), ptr(fwd, f64), ptr(tb, i64)))
+        self.check(self.lib.tb2_banded_forward_pass(self.handle, ptr(z, f64), ptr(es, i64), nb, bw,
+                                                    skip_pen, stay_pen, ptr(fwd, f64),
+                                                    ptr(tb, i64)))
         return fwd, tb
 
     def banded_traceback(self, tb, event_starts, band_pos, thresh=-1):
@@ -294,11 +351,9 @@ class Context(object):
         nb = tb.shape[0] - 1
         out = np.empty(nb + 1, dtype=np.int64)
         st = C.c_int(0)
-        fn = self.lib.tb2_banded_traceback
-        fn.restype = C.c_int
-        self.check(fn(self.handle, ptr(tb, i64), ptr(es, i64), i64(nb),
-                      i64(tb.shape[1]), i64(int(band_pos)), i64(int(thresh)),
-                      ptr(out, i64), C.byref(st)))
+        self.check(self.lib.tb2_banded_traceback(self.handle, ptr(tb, i64), ptr(es, i64), nb,
+                                                 tb.shape[1], int(band_pos), int(thresh),
+                                                 ptr(out, i64), C.byref(st)))
         return st.value, out
 
     def adaptive_banded_forward_pass(self, fwd, tb, event_starts, event_means,
@@ -310,15 +365,11 @@ class Context(object):
         assert event_starts.flags.c_contiguous and event_starts.dtype == np.int64
         em, rm, rs = as_f64(event_means), as_f64(rm), as_f64(rs)
         st = C.c_int(0)
-        fn = self.lib.tb2_adaptive_banded_forward_pass
-        fn.restype = C.c_int
-        self.check(fn(self.handle, ptr(fwd, f64), ptr(tb, i64),
-                      ptr(event_starts, i64), i64(fwd.shape[0] - 1),
-                      i64(fwd.shape[1]), ptr(em, f64), i64(em.shape[0]),
-                      ptr(rm, f64), ptr(rs, f64), f64(z_shift), f64(skip_pen),
-                      f64(stay_pen), i64(start_seq_pos), f64(mask_fill_z),
-                      C.c_int(int(bool(do_winsorize))), f64(max_half_z),
-                      C.byref(st)))
+        self.check(self.lib.tb2_adaptive_banded_forward_pass(
+            self.handle, ptr(fwd, f64), ptr(tb, i64), ptr(event_starts, i64), fwd.shape[0] - 1,
+            fwd.shape[1], ptr(em, f64), em.shape[0], ptr(rm, f64), ptr(rs, f64), z_shift,
+            skip_pen, stay_pen, int(start_seq_pos), mask_fill_z, int(bool(do_winsorize)),
+            max_half_z, C.byref(st)))
         return st.value
 
     def find_adaptive_base_assignment(self, valid_cpts, event_means, params,
@@ -331,12 +382,10 @@ class Context(object):
         dbg = np.zeros(3, dtype=np.int64)
         st = C.c_int(0)
         p = params if isinstance(params, Params) else params_struct(params)
-        fn = self.lib.tb2_find_adaptive_base_assignment
-        fn.restype = C.c_int
-        self.check(fn(self.handle, ptr(cp, i64), i64(cp.shape[0]), ptr(em, f64),
-                      C.byref(p), ptr(rm, f64), ptr(rs, f64), i64(nb),
-                      f64(sig_match_thresh), ptr(segs, i64), C.byref(rsrtr),
-                      ptr(dbg, i64), C.byref(st)))
+        self.check(self.lib.tb2_find_adaptive_base_assignment(
+            self.handle, ptr(cp, i64), cp.shape[0], ptr(em, f64), C.byref(p), ptr(rm, f64),
+            ptr(rs, f64), nb, sig_match_thresh, ptr(segs, i64), C.byref(rsrtr), ptr(dbg, i64),
+            C.byref(st)))
         return st.value, segs, rsrtr.value, dbg
 
 
@@ -344,38 +393,31 @@ class Context(object):
     def set_model(self, means, sds, kmer_width, central_pos):
         means, sds = as_f64(means), as_f64(sds)
         assert means.shape[0] == 4 ** kmer_width == sds.shape[0]
-        fn = self.lib.tb2_set_model
-        fn.restype = C.c_int
         self._model_ref = self._model_digest = None     # ensure_model uploads next time
-        self.check(fn(self.handle, ptr(means, f64), ptr(sds, f64),
-                      C.c_int(kmer_width), C.c_int(central_pos)))
+        self.check(self.lib.tb2_set_model(self.handle, ptr(means, f64), ptr(sds, f64),
+                                          int(kmer_width), int(central_pos)))
         self.kmer_width, self.central_pos = kmer_width, central_pos
 
     def set_alt_model(self, alt_means, kmer_width):
         alt_means = as_f64(alt_means)
         assert alt_means.size == 4 ** kmer_width * kmer_width
-        fn = self.lib.tb2_set_alt_model
-        fn.restype = C.c_int
-        self.check(fn(self.handle, ptr(alt_means, f64), C.c_int(kmer_width)))
+        self.check(self.lib.tb2_set_alt_model(self.handle, ptr(alt_means, f64), int(kmer_width)))
 
     # ---- mirror API: _c_helper.pyx / tombo_stats.py ------------------------
     def new_means(self, sig, segs):
         sig, segs = as_f64(sig), as_i64(segs)
         out = np.empty(segs.shape[0] - 1)
-        fn = self.lib.tb2_new_means
-        fn.restype = C.c_int
-        self.check(fn(self.handle, ptr(sig, f64), i64(sig.shape[0]), ptr(segs, i64),
-                      i64(out.shape[0]), ptr(out, f64)))
+        self.check(self.lib.tb2_new_means(self.handle, ptr(sig, f64), sig.shape[0], ptr(segs, i64),
+                                          out.shape[0], ptr(out, f64)))
         return out
 
     def new_mean_stds(self, sig, segs):
         sig, segs = as_f64(sig), as_i64(segs)
         m = np.empty(segs.shape[0] - 1)
         sd = np.empty(segs.shape[0] - 1)
-        fn = self.lib.tb2_new_mean_stds
-        fn.restype = C.c_int
-        self.check(fn(self.handle, ptr(sig, f64), i64(sig.shape[0]), ptr(segs, i64),
-                      i64(m.shape[0]), ptr(m, f64), ptr(sd, f64)))
+        self.check(self.lib.tb2_new_mean_stds(self.handle, ptr(sig, f64), sig.shape[0],
+                                              ptr(segs, i64), m.shape[0], ptr(m, f64),
+                                              ptr(sd, f64)))
         return m, sd
 
     def normalize_raw_signal(self, raw, outlier_thresh=None, scale_values=None,
@@ -387,14 +429,11 @@ class Context(object):
         if scale_values is not None:
             svi = ScaleValues(*[float('nan') if v is None else float(v)
                                 for v in scale_values])
-        fn = self.lib.tb2_normalize_raw_signal
-        fn.restype = C.c_int
-        st = fn(self.handle, ptr(raw, f64), i64(raw.shape[0]),
-                C.c_int(0 if const_scale is None else 1),
-                f64(float('nan') if outlier_thresh is None else outlier_thresh),
-                f64(float('nan') if const_scale is None else const_scale),
-                C.byref(svi) if svi is not None else None, ptr(norm, f64),
-                C.byref(sv))
+        st = self.lib.tb2_normalize_raw_signal(
+            self.handle, ptr(raw, f64), raw.shape[0], 0 if const_scale is None else 1,
+            float('nan') if outlier_thresh is None else outlier_thresh,
+            float('nan') if const_scale is None else const_scale,
+            C.byref(svi) if svi is not None else None, ptr(norm, f64), C.byref(sv))
         if st >= 200:
             self.check(st)
         return st, norm, (sv.shift, sv.scale, sv.lower_lim, sv.upper_lim,
@@ -405,22 +444,19 @@ class Context(object):
         sig = as_f64(sig)
         out = np.empty(num_cpts, dtype=np.int64)
         st = C.c_int(0)
-        fn = self.lib.tb2_valid_cpts_w_cap
-        fn.restype = C.c_int
-        self.check(fn(self.handle, ptr(sig, f64), i64(sig.shape[0]),
-                      i64(min_base_obs), i64(running_stat_width), i64(num_cpts),
-                      C.c_int(int(bool(t_test))), ptr(out, i64), C.byref(st)))
+        self.check(self.lib.tb2_valid_cpts_w_cap(self.handle, ptr(sig, f64), sig.shape[0],
+                                                 int(min_base_obs), int(running_stat_width),
+                                                 int(num_cpts), int(bool(t_test)), ptr(out, i64),
+                                                 C.byref(st)))
         return st.value, out
 
     def theil_sen(self, prev_shift, prev_scale, event_means, model_means, key=0):
         ev, md = as_f64(event_means), as_f64(model_means)
         out = np.empty(4)
         st = C.c_int(0)
-        fn = self.lib.tb2_theil_sen
-        fn.restype = C.c_int
-        self.check(fn(self.handle, f64(prev_shift), f64(prev_scale), ptr(ev, f64),
-                      ptr(md, f64), i64(ev.shape[0]), C.c_uint32(key),
-                      ptr(out, f64), C.byref(st)))
+        self.check(self.lib.tb2_theil_sen(self.handle, prev_shift, prev_scale, ptr(ev, f64),
+                                          ptr(md, f64), ev.shape[0], int(key), ptr(out, f64),
+                                          C.byref(st)))
         return st.value, tuple(out)
 
     def resolve_skipped_bases_with_raw(self, segs, rm, rs, norm, params,
@@ -429,13 +465,10 @@ class Context(object):
         out = np.empty_like(segs)
         st = C.c_int(0)
         p = params if isinstance(params, Params) else params_struct(params)
-        fn = self.lib.tb2_resolve_skipped_bases_with_raw
-        fn.restype = C.c_int
-        self.check(fn(self.handle, ptr(segs, i64), i64(segs.shape[0] - 1),
-                      ptr(rm, f64), ptr(rs, f64), ptr(norm, f64),
-                      i64(norm.shape[0]), C.byref(p),
-                      i64(-1 if max_raw_cpts is None else max_raw_cpts),
-                      ptr(out, i64), C.byref(st)))
+        self.check(self.lib.tb2_resolve_skipped_bases_with_raw(
+            self.handle, ptr(segs, i64), segs.shape[0] - 1, ptr(rm, f64), ptr(rs, f64),
+            ptr(norm, f64), norm.shape[0], C.byref(p),
+            -1 if max_raw_cpts is None else int(max_raw_cpts), ptr(out, i64), C.byref(st)))
         return st.value, out
 
     def identify_stalls(self, raw):
@@ -443,10 +476,8 @@ class Context(object):
         cap = raw.shape[0] // 200 + 4
         out = np.empty(2 * cap, dtype=np.int64)
         n = i64(0)
-        fn = self.lib.tb2_identify_stalls
-        fn.restype = C.c_int
-        self.check(fn(self.handle, ptr(raw, f64), i64(raw.shape[0]), ptr(out, i64),
-                      i64(cap), C.byref(n)))
+        self.check(self.lib.tb2_identify_stalls(self.handle, ptr(raw, f64), raw.shape[0],
+                                                ptr(out, i64), cap, C.byref(n)))
         return out[:2 * n.value].reshape(-1, 2).copy()
 
     def calc_llh_ratio_windows(self, mode, means, ref_means, alt_means, var_a, var_b=None,
@@ -456,12 +487,10 @@ class Context(object):
         n, k = means.shape
         out = np.empty(n)
         vb = as_f64(var_b) if var_b is not None else None
-        fn = self.lib.tb2_calc_llh_ratio_windows
-        fn.restype = C.c_int
-        self.check(fn(self.handle, C.c_int(mode), i64(n), C.c_int(k), ptr(means, f64),
-                      ptr(ref_means, f64), ptr(alt_means, f64), ptr(var_a, f64),
-                      ptr(vb, f64) if vb is not None else None, f64(scale_factor),
-                      f64(height_factor), f64(height_power), ptr(out, f64)))
+        self.check(self.lib.tb2_calc_llh_ratio_windows(
+            self.handle, int(mode), n, k, ptr(means, f64), ptr(ref_means, f64),
+            ptr(alt_means, f64), ptr(var_a, f64), ptr(vb, f64) if vb is not None else None,
+            scale_factor, height_factor, height_power, ptr(out, f64)))
         return out
 
     def find_static_base_assignment(self, event_means, rm, rs, params):
@@ -469,10 +498,9 @@ class Context(object):
         out = np.empty(rm.shape[0] + 1, dtype=np.int64)
         st = C.c_int(0)
         p = params if isinstance(params, Params) else params_struct(params)
-        fn = self.lib.tb2_find_static_base_assignment
-        fn.restype = C.c_int
-        self.check(fn(self.handle, ptr(em, f64), i64(em.shape[0]), ptr(rm, f64), ptr(rs, f64),
-                      i64(rm.shape[0]), C.byref(p), ptr(out, i64), C.byref(st)))
+        self.check(self.lib.tb2_find_static_base_assignment(
+            self.handle, ptr(em, f64), em.shape[0], ptr(rm, f64), ptr(rs, f64), rm.shape[0],
+            C.byref(p), ptr(out, i64), C.byref(st)))
         return st.value, out
 
     def find_seq_start_in_events(self, event_means, rm, rs, params, num_bases, num_events,
@@ -480,13 +508,11 @@ class Context(object):
         em, rm, rs = as_f64(event_means), as_f64(rm), as_f64(rs)
         st, sl, epb = C.c_int(0), i64(0), f64(0)
         p = params if isinstance(params, Params) else params_struct(params)
-        fn = self.lib.tb2_find_seq_start_in_events
-        fn.restype = C.c_int
-        self.check(fn(self.handle, ptr(em, f64), i64(em.shape[0]), ptr(rm, f64), ptr(rs, f64),
-                      i64(rm.shape[0]), C.byref(p), i64(num_bases), i64(num_events),
-                      C.c_int(int(sig_match_thresh is not None)),
-                      f64(0.0 if sig_match_thresh is None else sig_match_thresh),
-                      C.byref(sl), C.byref(epb), C.byref(st)))
+        self.check(self.lib.tb2_find_seq_start_in_events(
+            self.handle, ptr(em, f64), em.shape[0], ptr(rm, f64), ptr(rs, f64), rm.shape[0],
+            C.byref(p), int(num_bases), int(num_events), int(sig_match_thresh is not None),
+            0.0 if sig_match_thresh is None else sig_match_thresh, C.byref(sl), C.byref(epb),
+            C.byref(st)))
         return st.value, sl.value, epb.value
 
     def batch_set_read_inputs(self, scale_values=None, stall_ints=None):
@@ -505,11 +531,10 @@ class Context(object):
                 for a, b in s:
                     flat[2 * k], flat[2 * k + 1] = a, b
                     k += 1
-        fn = self.lib.tb2_batch_set_read_inputs
-        fn.restype = C.c_int
-        self.check(fn(self.handle, sv.ctypes.data_as(C.c_void_p) if sv is not None else None,
-                      ptr(flat, i64) if flat is not None else None,
-                      ptr(off, i64) if off is not None else None))
+        self.check(self.lib.tb2_batch_set_read_inputs(
+            self.handle, ptr(sv, ScaleValues) if sv is not None else None,
+            ptr(flat, i64) if flat is not None else None,
+            ptr(off, i64) if off is not None else None))
 
     # ---- the batched hot path ----------------------------------------------
     def resquiggle_batch(self, raw, raw_off, seq, seq_off, params, save_params,
@@ -524,44 +549,18 @@ class Context(object):
             dtype = 0
         raw_off, seq_off = as_i64(raw_off), as_i64(seq_off)
         seq = np.ascontiguousarray(seq, dtype=np.uint8)
-        n = raw_off.shape[0] - 1
-        k = self.kmer_width
-        # sequences shorter than the k-mer map zero bases (the library clamps the same way)
-        nb = np.maximum((seq_off[1:] - seq_off[:-1]) - (k - 1), 0)
-        base_off = np.concatenate([[0], np.cumsum(nb)]).astype(np.int64)
-        seg_off = base_off + np.arange(n + 1, dtype=np.int64)
+        base_off, seg_off = _offsets(seq_off, self.kmer_width)
         if out is None:
             out = {}
-        def buf(name, shape, dt):
-            a = out.get(name)
-            if a is None or a.shape != tuple(np.atleast_1d(shape)) or a.dtype != dt:
-                a = out[name] = np.empty(shape, dtype=dt)
-            return a
-        segs = buf('segs', int(seg_off[-1]), np.int64)
-        rsrtr = buf('read_start_rel_to_raw', n, np.int64)
-        sv = buf('scale_values', (n, 5), np.float64)
-        score = buf('sig_match_score', n, np.float64)
-        norm_mean = buf('norm_mean', int(base_off[-1]), np.float64)
-        status = buf('status', n, np.int32)
-        n_iters = buf('n_iters', n, np.int32)
-        flags = buf('flags', n, np.int32)
-        norm_sig = buf('norm_signal', raw.shape[0], np.float64) if want_norm_signal else None
+        outs = _batch_outputs(out, base_off, seg_off, raw.shape[0], want_norm_signal)
         p = params if isinstance(params, Params) else params_struct(params)
         sp = None
         if save_params is not None:
             sp = save_params if isinstance(save_params, Params) else params_struct(save_params)
-        fn = self.lib.tb2_resquiggle_batch
-        fn.restype = C.c_int
-        self.check(fn(self.handle, i64(n), raw.ctypes.data_as(C.c_void_p),
-                      C.c_int(dtype), ptr(raw_off, i64), ptr(seq, C.c_uint8),
-                      ptr(seq_off, i64), C.byref(p),
-                      C.byref(sp) if sp is not None else None, C.byref(policy),
-                      ptr(segs, i64), ptr(rsrtr, i64),
-                      sv.ctypes.data_as(C.c_void_p), ptr(score, f64),
-                      ptr(norm_mean, f64),
-                      ptr(norm_sig, f64) if norm_sig is not None else None,
-                      ptr(status, C.c_int32), ptr(n_iters, C.c_int32),
-                      ptr(flags, C.c_int32)))
+        self.check(self.lib.tb2_resquiggle_batch(
+            self.handle, raw_off.shape[0] - 1, raw.ctypes.data_as(C.c_void_p), dtype,
+            ptr(raw_off, i64), ptr(seq, C.c_uint8), ptr(seq_off, i64), C.byref(p),
+            C.byref(sp) if sp is not None else None, C.byref(policy), *outs))
         out['base_off'], out['seg_off'] = base_off, seg_off
         return out
 
@@ -576,13 +575,11 @@ class Context(object):
         llr = np.empty(cap)
         pos = np.empty(cap, dtype=np.int64)
         site_off = np.zeros(n + 1, dtype=np.int64)
-        fn = self.lib.tb2_alt_model_llr_batch
-        fn.restype = C.c_int
-        self.check(fn(self.handle, i64(n), ptr(norm_mean, f64), ptr(mean_off, i64),
-                      ptr(seq, C.c_uint8), ptr(seq_off, i64), ptr(read_start, i64),
-                      C.c_int(alt_base_code), C.c_int(int(bool(use_standard_llhr))),
-                      f64(scale_factor), f64(height_factor), f64(height_power),
-                      ptr(llr, f64), ptr(pos, i64), ptr(site_off, i64)))
+        self.check(self.lib.tb2_alt_model_llr_batch(
+            self.handle, n, ptr(norm_mean, f64), ptr(mean_off, i64), ptr(seq, C.c_uint8),
+            ptr(seq_off, i64), ptr(read_start, i64), int(alt_base_code),
+            int(bool(use_standard_llhr)), scale_factor, height_factor, height_power,
+            ptr(llr, f64), ptr(pos, i64), ptr(site_off, i64)))
         tot = int(site_off[-1])
         return llr[:tot].copy(), pos[:tot].copy(), site_off
 
@@ -593,11 +590,9 @@ class Context(object):
         """LLRs of the resident batch (after batch_compute); returns the site count"""
         read_start = as_i64(read_start)
         tot = i64(0)
-        fn = self.lib.tb2_batch_alt_llr
-        fn.restype = C.c_int
-        self.check(fn(self.handle, ptr(read_start, i64), C.c_int(alt_base_code),
-                      C.c_int(int(bool(use_standard_llhr))), f64(scale_factor),
-                      f64(height_factor), f64(height_power), C.byref(tot)))
+        self.check(self.lib.tb2_batch_alt_llr(self.handle, ptr(read_start, i64), int(alt_base_code),
+                                              int(bool(use_standard_llhr)), scale_factor,
+                                              height_factor, height_power, C.byref(tot)))
         self._llr_total, self._llr_reads = int(tot.value), read_start.shape[0]
         return self._llr_total
 
@@ -617,15 +612,12 @@ class Context(object):
         pos = np.empty(cap, dtype=np.int64)
         site_off = np.zeros(n + 1, dtype=np.int64)
         status = np.zeros(max(1, n), dtype=np.int32)
-        fn = self.lib.tb2_alt_model_llr_motif_batch
-        fn.restype = C.c_int
-        self.check(fn(self.handle, i64(n), ptr(norm_mean, f64), ptr(mean_off, i64),
-                      ptr(seq, C.c_uint8), ptr(seq_off, i64), ptr(read_start, i64),
-                      ptr(strand, C.c_int8), C.byref(motif), i64(int(max_motif_bb)),
-                      i64(int(max_motif_ab)), i64(int(reg_start)), i64(int(reg_end)),
-                      C.c_int(int(bool(use_standard_llhr))), f64(scale_factor),
-                      f64(height_factor), f64(height_power), ptr(llr, f64), ptr(pos, i64),
-                      ptr(site_off, i64), ptr(status, C.c_int32)))
+        self.check(self.lib.tb2_alt_model_llr_motif_batch(
+            self.handle, n, ptr(norm_mean, f64), ptr(mean_off, i64), ptr(seq, C.c_uint8),
+            ptr(seq_off, i64), ptr(read_start, i64), ptr(strand, C.c_int8), C.byref(motif),
+            int(max_motif_bb), int(max_motif_ab), int(reg_start), int(reg_end),
+            int(bool(use_standard_llhr)), scale_factor, height_factor, height_power,
+            ptr(llr, f64), ptr(pos, i64), ptr(site_off, i64), ptr(status, C.c_int32)))
         tot = int(site_off[-1])
         return llr[:tot].copy(), pos[:tot].copy(), site_off, status[:n].copy()
 
@@ -642,13 +634,11 @@ class Context(object):
                              'batch (%d)' % n)
         status = np.zeros(max(1, n), dtype=np.int32)
         tot = i64(0)
-        fn = self.lib.tb2_batch_alt_llr_motif
-        fn.restype = C.c_int
-        self.check(fn(self.handle, ptr(read_start, i64), ptr(strand, C.c_int8), C.byref(motif),
-                      i64(int(max_motif_bb)), i64(int(max_motif_ab)), i64(int(reg_start)),
-                      i64(int(reg_end)), C.c_int(int(bool(use_standard_llhr))),
-                      f64(scale_factor), f64(height_factor), f64(height_power),
-                      ptr(status, C.c_int32), C.byref(tot)))
+        self.check(self.lib.tb2_batch_alt_llr_motif(
+            self.handle, ptr(read_start, i64), ptr(strand, C.c_int8), C.byref(motif),
+            int(max_motif_bb), int(max_motif_ab), int(reg_start), int(reg_end),
+            int(bool(use_standard_llhr)), scale_factor, height_factor, height_power,
+            ptr(status, C.c_int32), C.byref(tot)))
         self._llr_total, self._llr_reads = int(tot.value), read_start.shape[0]
         return self._llr_total, status[:read_start.shape[0]].copy()
 
@@ -656,46 +646,34 @@ class Context(object):
         llr = np.empty(max(1, self._llr_total))
         pos = np.empty(max(1, self._llr_total), dtype=np.int64)
         site_off = np.zeros(self._llr_reads + 1, dtype=np.int64)
-        fn = self.lib.tb2_batch_llr_download
-        fn.restype = C.c_int
-        self.check(fn(self.handle, ptr(llr, f64), ptr(pos, i64), ptr(site_off, i64)))
+        self.check(self.lib.tb2_batch_llr_download(self.handle, ptr(llr, f64), ptr(pos, i64),
+                                                   ptr(site_off, i64)))
         return llr[:self._llr_total], pos[:self._llr_total], site_off
 
     def region_stats_begin(self, reg_start, reg_len):
-        fn = self.lib.tb2_region_stats_begin
-        fn.restype = C.c_int
-        self.check(fn(self.handle, i64(int(reg_start)), i64(int(reg_len))))
+        self.check(self.lib.tb2_region_stats_begin(self.handle, int(reg_start), int(reg_len)))
         self._reg_len = int(reg_len)
 
     def region_stats_add(self, stats, pos, single_read_thresh, lower_thresh=None, stat_type=0):
         stats, pos = as_f64(stats), as_i64(pos)
-        fn = self.lib.tb2_region_stats_add
-        fn.restype = C.c_int
-        self.check(fn(self.handle, i64(stats.shape[0]), ptr(stats, f64), ptr(pos, i64),
-                      f64(single_read_thresh),
-                      f64(float('nan') if lower_thresh is None else lower_thresh),
-                      C.c_int(stat_type)))
+        self.check(self.lib.tb2_region_stats_add(
+            self.handle, stats.shape[0], ptr(stats, f64), ptr(pos, i64), single_read_thresh,
+            float('nan') if lower_thresh is None else lower_thresh, int(stat_type)))
 
     def region_stats_add_batch_llr(self, single_read_thresh, lower_thresh=None, stat_type=0):
-        fn = self.lib.tb2_region_stats_add_batch_llr
-        fn.restype = C.c_int
-        self.check(fn(self.handle, f64(single_read_thresh),
-                      f64(float('nan') if lower_thresh is None else lower_thresh),
-                      C.c_int(stat_type)))
+        self.check(self.lib.tb2_region_stats_add_batch_llr(
+            self.handle, single_read_thresh,
+            float('nan') if lower_thresh is None else lower_thresh, int(stat_type)))
 
     def region_counts_get(self):
         cnt = np.zeros(3 * self._reg_len, dtype=np.int32)
-        fn = self.lib.tb2_region_counts_get
-        fn.restype = C.c_int
-        self.check(fn(self.handle, ptr(cnt, C.c_int32)))
+        self.check(self.lib.tb2_region_counts_get(self.handle, ptr(cnt, C.c_int32)))
         return cnt
 
     def region_counts_set(self, counts):
         cnt = np.ascontiguousarray(counts, dtype=np.int32)
         assert cnt.shape[0] == 3 * self._reg_len
-        fn = self.lib.tb2_region_counts_set
-        fn.restype = C.c_int
-        self.check(fn(self.handle, ptr(cnt, C.c_int32)))
+        self.check(self.lib.tb2_region_counts_set(self.handle, ptr(cnt, C.c_int32)))
 
     def region_stats_finalize(self, unmod_count=None, mod_count=None):
         cap = self._reg_len
@@ -703,11 +681,10 @@ class Context(object):
         frac, damp = np.empty(cap), np.empty(cap)
         cov, valid = np.empty(cap, dtype=np.int64), np.empty(cap, dtype=np.int64)
         n = i64(0)
-        fn = self.lib.tb2_region_stats_finalize
-        fn.restype = C.c_int
-        self.check(fn(self.handle, f64(float('nan') if unmod_count is None else unmod_count),
-                      f64(0.0 if mod_count is None else mod_count), i64(cap), ptr(pos, i64),
-                      ptr(frac, f64), ptr(damp, f64), ptr(cov, i64), ptr(valid, i64), C.byref(n)))
+        self.check(self.lib.tb2_region_stats_finalize(
+            self.handle, float('nan') if unmod_count is None else unmod_count,
+            0.0 if mod_count is None else mod_count, cap, ptr(pos, i64), ptr(frac, f64),
+            ptr(damp, f64), ptr(cov, i64), ptr(valid, i64), C.byref(n)))
         m = int(n.value)
         return dict(pos=pos[:m].copy(), frac=frac[:m].copy(), damp_frac=damp[:m].copy(),
                     cov=cov[:m].copy(), valid_cov=valid[:m].copy())
@@ -716,16 +693,14 @@ class Context(object):
         means = as_f64(means)
         seg_off = as_i64(seg_off)
         out = np.empty(max(1, means.shape[0]))
-        fn = self.lib.tb2_window_fisher_pvals
-        fn.restype = C.c_int
         if ref_means is None:            # `means` are p-values: Fisher window only
             prm = prs = None
         else:
             ref_means, ref_sds = as_f64(ref_means), as_f64(ref_sds)
             prm, prs = ptr(ref_means, f64), ptr(ref_sds, f64)
-        self.check(fn(self.handle, i64(seg_off.shape[0] - 1), ptr(means, f64), prm,
-                      prs, ptr(seg_off, i64), i64(int(fm_offset)),
-                      C.c_int(int(bool(final_clamp))), ptr(out, f64)))
+        self.check(self.lib.tb2_window_fisher_pvals(
+            self.handle, seg_off.shape[0] - 1, ptr(means, f64), prm, prs, ptr(seg_off, i64),
+            int(fm_offset), int(bool(final_clamp)), ptr(out, f64)))
         return out[:means.shape[0]]
 
     def group_reg_stats(self, reg_start, reg_len, samp, ctrl, test, return_stat, min_test_reads,
@@ -738,14 +713,11 @@ class Context(object):
         pos, stat = np.empty(cap, dtype=np.int64), np.empty(cap)
         cov, ccov = np.empty(cap, dtype=np.int64), np.empty(cap, dtype=np.int64)
         n = i64(0)
-        fn = self.lib.tb2_group_reg_stats
-        fn.restype = C.c_int
-        self.check(fn(self.handle, i64(int(reg_start)), i64(cap), i64(so.shape[0] - 1),
-                      ptr(sl, f64), ptr(so, i64), ptr(ss, i64), i64(co.shape[0] - 1),
-                      ptr(cl, f64), ptr(co, i64), ptr(cs, i64), C.c_int(int(test)),
-                      C.c_int(int(bool(return_stat))), i64(int(min_test_reads)),
-                      i64(int(fm_offset)), i64(cap), ptr(pos, i64), ptr(stat, f64),
-                      ptr(cov, i64), ptr(ccov, i64), C.byref(n)))
+        self.check(self.lib.tb2_group_reg_stats(
+            self.handle, int(reg_start), cap, so.shape[0] - 1, ptr(sl, f64), ptr(so, i64),
+            ptr(ss, i64), co.shape[0] - 1, ptr(cl, f64), ptr(co, i64), ptr(cs, i64), int(test),
+            int(bool(return_stat)), int(min_test_reads), int(fm_offset), cap, ptr(pos, i64),
+            ptr(stat, f64), ptr(cov, i64), ptr(ccov, i64), C.byref(n)))
         m = int(n.value)
         return dict(pos=pos[:m].copy(), stat=stat[:m].copy(), cov=cov[:m].copy(),
                     ctrl_cov=ccov[:m].copy())
@@ -762,13 +734,11 @@ class Context(object):
             if prior_means.shape[0] != n or prior_sds.shape[0] != n:
                 raise ValueError('prior levels must cover the region')
             pm, ps = ptr(prior_means, f64), ptr(prior_sds, f64)
-        fn = self.lib.tb2_reads_ref_levels
-        fn.restype = C.c_int
-        self.check(fn(self.handle, i64(int(reg_start)), i64(n), i64(off.shape[0] - 1),
-                      ptr(lv, f64), ptr(off, i64), ptr(st, i64), i64(int(min_test_reads)),
-                      C.c_int(int(bool(est_mean))), pm, ps, f64(float(prior_weights[0])),
-                      f64(float(prior_weights[1])), ptr(means, f64), ptr(sds, f64),
-                      ptr(cov, i64)))
+        self.check(self.lib.tb2_reads_ref_levels(
+            self.handle, int(reg_start), n, off.shape[0] - 1, ptr(lv, f64), ptr(off, i64),
+            ptr(st, i64), int(min_test_reads), int(bool(est_mean)), pm, ps,
+            float(prior_weights[0]), float(prior_weights[1]), ptr(means, f64), ptr(sds, f64),
+            ptr(cov, i64)))
         return means, sds, cov
 
     def de_novo_read_stats_batch(self, norm_mean, mean_off, seq, seq_off, read_start, fm_offset=1):
@@ -780,11 +750,10 @@ class Context(object):
         pv = np.empty(cap)
         pos = np.empty(cap, dtype=np.int64)
         stat_off = np.zeros(n + 1, dtype=np.int64)
-        fn = self.lib.tb2_de_novo_read_stats_batch
-        fn.restype = C.c_int
-        self.check(fn(self.handle, i64(n), ptr(norm_mean, f64), ptr(mean_off, i64),
-                      ptr(seq, C.c_uint8), ptr(seq_off, i64), ptr(read_start, i64),
-                      i64(int(fm_offset)), ptr(pv, f64), ptr(pos, i64), ptr(stat_off, i64)))
+        self.check(self.lib.tb2_de_novo_read_stats_batch(
+            self.handle, n, ptr(norm_mean, f64), ptr(mean_off, i64), ptr(seq, C.c_uint8),
+            ptr(seq_off, i64), ptr(read_start, i64), int(fm_offset), ptr(pv, f64), ptr(pos, i64),
+            ptr(stat_off, i64)))
         t = int(stat_off[-1])
         return pv[:t].copy(), pos[:t].copy(), stat_off
 

@@ -5,6 +5,7 @@
 #include "../../include/tombo_b200.h"
 struct tb2_ctx;
 #else
+#include <climits>
 #include "ctx.h"
 #endif
 
@@ -108,3 +109,41 @@ struct BatchResultView {
 int tb2_batch_result_view(tb2_ctx *ctx, BatchResultView *out);
 int tb2_region_accumulate_dev(tb2_ctx *ctx, long long n, const double *stats_dev,
                               const long long *pos_dev, double thresh, double lower, int stat_type);
+
+#ifndef TB2_EMUL
+// Reads in host arrays (tb2_alt_model_llr_batch, tb2_alt_model_llr_motif_batch,
+// tb2_de_novo_read_stats_batch): read r holds nb = mean_off[r + 1] - mean_off[r] means and
+// the nb + K - 1 base codes of their k-mers at seq_off[r].  Checks that layout, with
+// n_reads and every nb at most INT_MAX (the kernels index reads and bases with int), before
+// reading any array past its first entry.  Then uploads the five arrays into buf[0..4] in
+// argument order and points the read arrays of `a` (LlrArgs or FisherArgs) at them.
+template <class Args>
+int tb2_stage_reads(tb2_ctx *ctx, int64_t n_reads, const double *norm_mean, const int64_t *mean_off,
+                    const uint8_t *seq, const int64_t *seq_off, const int64_t *read_start,
+                    DevBuf buf[5], Args &a)
+{
+    if (n_reads < 0 || n_reads > INT_MAX || !mean_off || !seq_off || !read_start)
+        return TB2_ERR_INVALID_ARG;
+    const int n = (int)n_reads;
+    if (mean_off[0] < 0 || seq_off[0] < 0) return TB2_ERR_INVALID_ARG;
+    for (int r = 0; r < n; ++r) {
+        const long long nb = mean_off[r + 1] - mean_off[r];
+        if (nb < 0 || nb > INT_MAX || seq_off[r + 1] - seq_off[r] != nb + (ctx->kmer_width - 1))
+            return TB2_ERR_INVALID_ARG;
+    }
+    const size_t tm = (size_t)mean_off[n], ts = (size_t)seq_off[n];
+    if ((tm && !norm_mean) || (ts && !seq)) return TB2_ERR_INVALID_ARG;
+    cudaStream_t s = ctx->stream;
+    TB2_CUDA_TRY(ctx, buf[0].upload(norm_mean, tm, s));
+    TB2_CUDA_TRY(ctx, buf[1].upload(mean_off, (size_t)n + 1, s));
+    TB2_CUDA_TRY(ctx, buf[2].upload(seq, ts, s));
+    TB2_CUDA_TRY(ctx, buf[3].upload(seq_off, (size_t)n + 1, s));
+    TB2_CUDA_TRY(ctx, buf[4].upload(read_start, (size_t)n, s));
+    a.norm_mean = buf[0].as<double>();
+    a.mean_off = buf[1].as<long long>();
+    a.seq = buf[2].as<unsigned char>();
+    a.seq_off = buf[3].as<long long>();
+    a.read_start = buf[4].as<long long>();
+    return TB2_OK;
+}
+#endif

@@ -30,6 +30,14 @@ struct DevBuf {
         if (e == cudaSuccess) cap = want;
         return e;
     }
+    // count elements of T from the host, enqueued on s.  The 8 spare bytes keep an empty
+    // upload on a valid pointer; an empty upload copies nothing, so host may then be null.
+    template <class T> cudaError_t upload(const T *host, size_t count, cudaStream_t s)
+    {
+        cudaError_t e = reserve(count * sizeof(T) + 8);
+        if (e != cudaSuccess || count == 0) return e;
+        return cudaMemcpyAsync(p, host, count * sizeof(T), cudaMemcpyHostToDevice, s);
+    }
     bool owned = true;   // false: alias of another context's buffer (pipeline lanes)
     void release()
     {

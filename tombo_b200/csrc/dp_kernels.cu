@@ -195,8 +195,8 @@ extern "C" int tb2_banded_forward_pass(tb2_ctx *ctx, const double *z, const int6
     if (tb2_row_cells(bw) / 32 > TB2_MAX_WPL * 16) return TB2_ERR_CAPACITY;
     const size_t nz = (size_t)n_bases * bw, nf = (size_t)(n_bases + 1) * bw;
     auto &P = tb2_state(ctx->dp).buf;
-    TB2_CUDA_TRY(ctx, P[S_A].reserve(nz * 8));
-    TB2_CUDA_TRY(ctx, P[S_B].reserve(n_bases * 8));
+    TB2_CUDA_TRY(ctx, P[S_A].upload(z, nz, ctx->stream));
+    TB2_CUDA_TRY(ctx, P[S_B].upload(event_starts, (size_t)n_bases, ctx->stream));
     TB2_CUDA_TRY(ctx, P[S_C].reserve(nf * 8));
     TB2_CUDA_TRY(ctx, P[S_D].reserve(nf * 8));
     TB2_CUDA_TRY(ctx, P[S_E].reserve(n_bases * 4));
@@ -204,9 +204,6 @@ extern "C" int tb2_banded_forward_pass(tb2_ctx *ctx, const double *z, const int6
     TB2_CUDA_TRY(ctx, P[S_G].reserve(4));
     const DbgGeom g = dbg_geom(bw);
     TB2_CUDA_TRY(ctx, P[S_H].reserve((size_t)g.grow_cells * 2 * 8 + 8));
-    TB2_CUDA_TRY(ctx, cudaMemcpyAsync(P[S_A].p, z, nz * 8, cudaMemcpyHostToDevice, ctx->stream));
-    TB2_CUDA_TRY(ctx, cudaMemcpyAsync(P[S_B].p, event_starts, n_bases * 8, cudaMemcpyHostToDevice,
-                                      ctx->stream));
     TB2_CUDA_TRY(ctx, cudaFuncSetAttribute(k_banded_forward_dbg,
                                            cudaFuncAttributeMaxDynamicSharedMemorySize,
                                            (int)g.smem_bytes));
@@ -233,13 +230,10 @@ extern "C" int tb2_banded_traceback(tb2_ctx *ctx, const int64_t *tb, const int64
     if (!tb || !event_starts || !seq_poss_out || n_bases < 1 || bw < 1) return TB2_ERR_INVALID_ARG;
     const size_t nf = (size_t)(n_bases + 1) * bw;
     auto &P = tb2_state(ctx->dp).buf;
-    TB2_CUDA_TRY(ctx, P[S_A].reserve(nf * 8));
-    TB2_CUDA_TRY(ctx, P[S_B].reserve(n_bases * 8));
+    TB2_CUDA_TRY(ctx, P[S_A].upload(tb, nf, ctx->stream));
+    TB2_CUDA_TRY(ctx, P[S_B].upload(event_starts, (size_t)n_bases, ctx->stream));
     TB2_CUDA_TRY(ctx, P[S_C].reserve((n_bases + 1) * 8));
     TB2_CUDA_TRY(ctx, P[S_G].reserve(4));
-    TB2_CUDA_TRY(ctx, cudaMemcpyAsync(P[S_A].p, tb, nf * 8, cudaMemcpyHostToDevice, ctx->stream));
-    TB2_CUDA_TRY(ctx, cudaMemcpyAsync(P[S_B].p, event_starts, n_bases * 8, cudaMemcpyHostToDevice,
-                                      ctx->stream));
     k_traceback_dbg<<<1, 32, 0, ctx->stream>>>(P[S_A].as<long long>(), P[S_B].as<long long>(),
                                                (int)n_bases, (int)bw, band_pos,
                                                band_boundary_thresh, P[S_C].as<long long>(),
@@ -268,24 +262,18 @@ extern "C" int tb2_adaptive_banded_forward_pass(
     if (tb2_row_cells(bw) / 32 > TB2_MAX_WPL * 16) return TB2_ERR_CAPACITY;
     const size_t nf = (size_t)(n_bases + 1) * bw;
     auto &P = tb2_state(ctx->dp).buf;
-    TB2_CUDA_TRY(ctx, P[S_A].reserve(nf * 8));
-    TB2_CUDA_TRY(ctx, P[S_B].reserve(nf * 8));
-    TB2_CUDA_TRY(ctx, P[S_C].reserve(n_bases * 8));
-    TB2_CUDA_TRY(ctx, P[S_D].reserve(n_events * 8));
-    TB2_CUDA_TRY(ctx, P[S_E].reserve(n_bases * 8));
-    TB2_CUDA_TRY(ctx, P[S_F].reserve(n_bases * 8));
+    cudaStream_t s = ctx->stream;
+    TB2_CUDA_TRY(ctx, P[S_A].upload(fwd, nf, s));
+    TB2_CUDA_TRY(ctx, P[S_B].upload(tb, nf, s));
+    TB2_CUDA_TRY(ctx, P[S_C].upload(event_starts, (size_t)n_bases, s));
+    TB2_CUDA_TRY(ctx, P[S_D].upload(event_means, (size_t)n_events, s));
+    TB2_CUDA_TRY(ctx, P[S_E].upload(ref_means, (size_t)n_bases, s));
+    TB2_CUDA_TRY(ctx, P[S_F].upload(ref_sds, (size_t)n_bases, s));
     TB2_CUDA_TRY(ctx, P[S_G].reserve(4));
     TB2_CUDA_TRY(ctx, P[S_I].reserve(n_bases * 4));
     TB2_CUDA_TRY(ctx, P[S_J].reserve((size_t)n_bases * TB2_MAX_WPL * 32 * 4));
     const DbgGeom g = dbg_geom(bw);
     TB2_CUDA_TRY(ctx, P[S_H].reserve((size_t)g.grow_cells * 2 * 8 + 8));
-    cudaStream_t s = ctx->stream;
-    TB2_CUDA_TRY(ctx, cudaMemcpyAsync(P[S_A].p, fwd, nf * 8, cudaMemcpyHostToDevice, s));
-    TB2_CUDA_TRY(ctx, cudaMemcpyAsync(P[S_B].p, tb, nf * 8, cudaMemcpyHostToDevice, s));
-    TB2_CUDA_TRY(ctx, cudaMemcpyAsync(P[S_C].p, event_starts, n_bases * 8, cudaMemcpyHostToDevice, s));
-    TB2_CUDA_TRY(ctx, cudaMemcpyAsync(P[S_D].p, event_means, n_events * 8, cudaMemcpyHostToDevice, s));
-    TB2_CUDA_TRY(ctx, cudaMemcpyAsync(P[S_E].p, ref_means, n_bases * 8, cudaMemcpyHostToDevice, s));
-    TB2_CUDA_TRY(ctx, cudaMemcpyAsync(P[S_F].p, ref_sds, n_bases * 8, cudaMemcpyHostToDevice, s));
     TB2_CUDA_TRY(ctx, cudaFuncSetAttribute(k_adaptive_dbg, cudaFuncAttributeMaxDynamicSharedMemorySize,
                                            (int)g.smem_bytes));
     k_adaptive_dbg<<<1, 32, g.smem_bytes, s>>>(
@@ -345,21 +333,16 @@ extern "C" int tb2_find_adaptive_base_assignment(
     for (int64_t i = 0; i < n_cpts; ++i) cp32[i] = (int)valid_cpts[i];
     long long offs[4] = {0, n_cpts, 0, nb};
     int ncp = (int)n_cpts, zero = 0;
-    TB2_CUDA_TRY(ctx, P[S_A].reserve(n_cpts * 4));
-    TB2_CUDA_TRY(ctx, P[S_B].reserve(n_cpts * 8));
-    TB2_CUDA_TRY(ctx, P[S_C].reserve(nb * 8));
-    TB2_CUDA_TRY(ctx, P[S_D].reserve(nb * 8));
-    TB2_CUDA_TRY(ctx, P[S_E].reserve(4 * 8));
+    TB2_CUDA_TRY(ctx, P[S_A].upload(cp32.data(), (size_t)n_cpts, s));
+    TB2_CUDA_TRY(ctx, P[S_B].upload(event_means, (size_t)n_em, s));
+    TB2_CUDA_TRY(ctx, P[S_C].upload(ref_means, (size_t)nb, s));
+    TB2_CUDA_TRY(ctx, P[S_D].upload(ref_sds, (size_t)nb, s));
+    TB2_CUDA_TRY(ctx, P[S_E].upload(offs, 4, s));
     TB2_CUDA_TRY(ctx, P[S_F].reserve((nb + 1) * 4 * 3 + 64));  // starts, read_tb, segs
-    TB2_CUDA_TRY(ctx, P[S_G].reserve(64));
-    TB2_CUDA_TRY(ctx, cudaMemcpyAsync(P[S_A].p, cp32.data(), n_cpts * 4, cudaMemcpyHostToDevice, s));
-    TB2_CUDA_TRY(ctx, cudaMemcpyAsync(P[S_B].p, event_means, n_em * 8, cudaMemcpyHostToDevice, s));
-    TB2_CUDA_TRY(ctx, cudaMemcpyAsync(P[S_C].p, ref_means, nb * 8, cudaMemcpyHostToDevice, s));
-    TB2_CUDA_TRY(ctx, cudaMemcpyAsync(P[S_D].p, ref_sds, nb * 8, cudaMemcpyHostToDevice, s));
-    TB2_CUDA_TRY(ctx, cudaMemcpyAsync(P[S_E].p, offs, 32, cudaMemcpyHostToDevice, s));
     // small ints: [0]=n_cpts [1]=status [2]=rsrtr [3..5]=dbg
     int small[8] = {ncp, zero, 0, 0, 0, 0, 0, 0};
-    TB2_CUDA_TRY(ctx, cudaMemcpyAsync(P[S_G].p, small, 32, cudaMemcpyHostToDevice, s));
+    TB2_CUDA_TRY(ctx, P[S_G].reserve(64));
+    TB2_CUDA_TRY(ctx, P[S_G].upload(small, 8, s));
     AlignBatch b;
     b.n_reads = 1;
     b.order = nullptr;
@@ -450,16 +433,13 @@ static int run_single(tb2_ctx *ctx, int mode, const double *em, int64_t n_em, co
     if (tb2_row_cells(W) / 32 > TB2_MAX_CHUNK) { if (read_status) *read_status = TB2_ERR_CAPACITY; return TB2_OK; }
     const DbgGeom g = dbg_geom(W);
     const size_t tbw = tb2_tb_words(rows, W, n_em);
-    TB2_CUDA_TRY(ctx, P[S_A].reserve((size_t)n_em * 8));
-    TB2_CUDA_TRY(ctx, P[S_B].reserve((size_t)nb * 8));
-    TB2_CUDA_TRY(ctx, P[S_C].reserve((size_t)nb * 8));
+    TB2_CUDA_TRY(ctx, P[S_A].upload(em, (size_t)n_em, s));
+    TB2_CUDA_TRY(ctx, P[S_B].upload(rm, (size_t)nb, s));
+    TB2_CUDA_TRY(ctx, P[S_C].upload(rs, (size_t)nb, s));
     TB2_CUDA_TRY(ctx, P[S_D].reserve((size_t)(nb + 1) * 4 * 2 + 64));
     TB2_CUDA_TRY(ctx, P[S_E].reserve(tbw * 4 + 64));
     TB2_CUDA_TRY(ctx, P[S_G].reserve(64));
     TB2_CUDA_TRY(ctx, P[S_H].reserve((size_t)g.grow_cells * 2 * 8 + 8));
-    TB2_CUDA_TRY(ctx, cudaMemcpyAsync(P[S_A].p, em, (size_t)n_em * 8, cudaMemcpyHostToDevice, s));
-    TB2_CUDA_TRY(ctx, cudaMemcpyAsync(P[S_B].p, rm, (size_t)nb * 8, cudaMemcpyHostToDevice, s));
-    TB2_CUDA_TRY(ctx, cudaMemcpyAsync(P[S_C].p, rs, (size_t)nb * 8, cudaMemcpyHostToDevice, s));
     TB2_CUDA_TRY(ctx, cudaFuncSetAttribute(k_single, cudaFuncAttributeMaxDynamicSharedMemorySize,
                                            (int)g.smem_bytes));
     int *ints = P[S_D].as<int>();

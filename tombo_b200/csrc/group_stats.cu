@@ -28,7 +28,7 @@ namespace {
 // per-call scratch of tb2_group_reg_stats / tb2_reads_ref_levels; nothing reads it after a
 // call returns
 enum { G_LV_S = 0, G_OFF_S, G_ST_S, G_LV_C, G_OFF_C, G_ST_C, G_INT, G_IDX, G_VAL, G_RD, G_SQ,
-       G_RES, G_PRI, G_REF, G_HDR, G_COUNT };
+       G_RES, G_PRI_M, G_PRI_S, G_REF, G_HDR, G_COUNT };
 }  // namespace
 struct GroupState { DevBuf scratch[G_COUNT]; };
 
@@ -386,14 +386,9 @@ int upload_sample(tb2_ctx *ctx, int slot, int64_t n, const double *lv, const int
     cudaStream_t q = ctx->stream;
     s.n = (int)n;
     s.total = n ? off[n] : 0;
-    TB2_CUDA_TRY(ctx, P[slot].reserve((size_t)s.total * 8 + 8));
-    TB2_CUDA_TRY(ctx, P[slot + 1].reserve((size_t)(n + 1) * 8));
-    TB2_CUDA_TRY(ctx, P[slot + 2].reserve((size_t)n * 8 + 8));
-    if (s.total) TB2_CUDA_TRY(ctx, cudaMemcpyAsync(P[slot].p, lv, (size_t)s.total * 8, cudaMemcpyHostToDevice, q));
-    if (n) {
-        TB2_CUDA_TRY(ctx, cudaMemcpyAsync(P[slot + 1].p, off, (size_t)(n + 1) * 8, cudaMemcpyHostToDevice, q));
-        TB2_CUDA_TRY(ctx, cudaMemcpyAsync(P[slot + 2].p, st, (size_t)n * 8, cudaMemcpyHostToDevice, q));
-    }
+    TB2_CUDA_TRY(ctx, P[slot].upload(lv, (size_t)s.total, q));
+    TB2_CUDA_TRY(ctx, P[slot + 1].upload(off, n ? (size_t)n + 1 : 0, q));   // off may be null when n == 0
+    TB2_CUDA_TRY(ctx, P[slot + 2].upload(st, (size_t)n, q));
     s.lv = P[slot].as<double>(); s.off = P[slot + 1].as<long long>(); s.st = P[slot + 2].as<long long>();
     return TB2_OK;
 }
@@ -534,10 +529,9 @@ extern "C" int tb2_reads_ref_levels(tb2_ctx *ctx, int64_t reg_start, int64_t reg
     const long long n = reg_len;
     const double *pm = nullptr, *ps = nullptr;
     if (prior_means) {
-        TB2_CUDA_TRY(ctx, P[G_PRI].reserve((size_t)n * 2 * 8));
-        TB2_CUDA_TRY(ctx, cudaMemcpyAsync(P[G_PRI].p, prior_means, (size_t)n * 8, cudaMemcpyHostToDevice, q));
-        TB2_CUDA_TRY(ctx, cudaMemcpyAsync(P[G_PRI].as<double>() + n, prior_sds, (size_t)n * 8, cudaMemcpyHostToDevice, q));
-        pm = P[G_PRI].as<double>(); ps = pm + n;
+        TB2_CUDA_TRY(ctx, P[G_PRI_M].upload(prior_means, (size_t)n, q));
+        TB2_CUDA_TRY(ctx, P[G_PRI_S].upload(prior_sds, (size_t)n, q));
+        pm = P[G_PRI_M].as<double>(); ps = P[G_PRI_S].as<double>();
     }
     long long hdr[4];
     if ((rc = gather(ctx, reg_start, reg_len, a, nullptr, (int)min_test_reads, 1, true, hdr))) return rc;

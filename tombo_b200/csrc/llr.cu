@@ -7,9 +7,7 @@
 // a region (the kernels are in motif_llr.cuh).  Also c_new_mean_stds :38-57.
 #include "batch.h"
 #include "motif_llr.cuh"
-#include <climits>
 #include <cstring>
-#include <vector>
 
 namespace {
 // per-call scratch of the entry points below; nothing reads it after a call returns
@@ -82,101 +80,7 @@ __global__ void k_mean_stds(const double *sig, const long long *segs, long long 
     for (long long k = a; k < z; ++k) { const double d = sig[k] - m; v += d * d; }
     sds[i] = sqrt(v / (double)(z - a));
 }
-}  // namespace
 
-extern "C" int tb2_set_alt_model(tb2_ctx *ctx, const double *alt_means, int kmer_width)
-{
-    int rc = tb2_use(ctx);
-    if (rc) return rc;
-    if (!alt_means || kmer_width < 1 || kmer_width > 12) return TB2_ERR_INVALID_ARG;
-    const size_t n = ((size_t)1 << (2 * kmer_width)) * kmer_width;
-    TB2_CUDA_TRY(ctx, ctx->alt_means.reserve(n * 8));
-    TB2_CUDA_TRY(ctx, cudaMemcpyAsync(ctx->alt_means.p, alt_means, n * 8, cudaMemcpyHostToDevice, ctx->stream));
-    TB2_CUDA_TRY(ctx, cudaStreamSynchronize(ctx->stream));
-    ctx->alt_kmer_width = kmer_width;
-    return TB2_OK;
-}
-
-extern "C" int tb2_alt_model_llr_batch(tb2_ctx *ctx, int64_t n_reads, const double *norm_mean,
-                                       const int64_t *mean_off, const uint8_t *seq,
-                                       const int64_t *seq_off, const int64_t *read_start,
-                                       int alt_base_code, int use_standard_llhr,
-                                       double scale_factor, double height_factor,
-                                       double height_power, double *llr_out, int64_t *pos_out,
-                                       int64_t *site_off)
-{
-    int rc = tb2_use(ctx);
-    if (rc) return rc;
-    if (n_reads < 0 || !mean_off || !seq_off || !read_start || !site_off || alt_base_code < 0 ||
-        alt_base_code > 3)
-        return TB2_ERR_INVALID_ARG;
-    if (ctx->kmer_width <= 0 || ctx->alt_kmer_width != ctx->kmer_width) {
-        ctx->err = "standard and alternative models must be set with the same k-mer width";
-        return TB2_ERR_INVALID_ARG;
-    }
-    site_off[0] = 0;
-    if (n_reads == 0) return TB2_OK;
-    if (!norm_mean || !seq || !llr_out || !pos_out) return TB2_ERR_INVALID_ARG;
-    const int n = (int)n_reads;
-    // every read holds nb means and the nb + K - 1 bases of their k-mers
-    for (int r = 0; r < n; ++r) {
-        const long long nb = mean_off[r + 1] - mean_off[r];
-        if (nb < 0 || seq_off[r + 1] - seq_off[r] != nb + (ctx->kmer_width - 1)) return TB2_ERR_INVALID_ARG;
-    }
-    auto &P = tb2_state(ctx->llr).scratch;
-    cudaStream_t s = ctx->stream;
-    const size_t tm = (size_t)mean_off[n], ts = (size_t)seq_off[n];
-    TB2_CUDA_TRY(ctx, P[L_MEAN].reserve(tm * 8 + 8));
-    TB2_CUDA_TRY(ctx, P[L_MOFF].reserve((n + 1) * 8));
-    TB2_CUDA_TRY(ctx, P[L_SEQ].reserve(ts + 8));
-    TB2_CUDA_TRY(ctx, P[L_SOFF].reserve((n + 1) * 8));
-    TB2_CUDA_TRY(ctx, P[L_START].reserve((size_t)n * 8));
-    TB2_CUDA_TRY(ctx, P[L_CNT].reserve((size_t)n * 4));
-    TB2_CUDA_TRY(ctx, P[L_SITEOFF].reserve((n + 1) * 8));
-    TB2_CUDA_TRY(ctx, cudaMemcpyAsync(P[L_MEAN].p, norm_mean, tm * 8, cudaMemcpyHostToDevice, s));
-    TB2_CUDA_TRY(ctx, cudaMemcpyAsync(P[L_MOFF].p, mean_off, (n + 1) * 8, cudaMemcpyHostToDevice, s));
-    TB2_CUDA_TRY(ctx, cudaMemcpyAsync(P[L_SEQ].p, seq, ts, cudaMemcpyHostToDevice, s));
-    TB2_CUDA_TRY(ctx, cudaMemcpyAsync(P[L_SOFF].p, seq_off, (n + 1) * 8, cudaMemcpyHostToDevice, s));
-    TB2_CUDA_TRY(ctx, cudaMemcpyAsync(P[L_START].p, read_start, (size_t)n * 8, cudaMemcpyHostToDevice, s));
-    LlrArgs a;
-    a.status = nullptr; a.status_stride = 0;
-    a.n_reads = n; a.K = ctx->kmer_width; a.cpos = ctx->central_pos; a.alt_code = alt_base_code;
-    a.use_std = use_standard_llhr ? 1 : 0;
-    a.sf = scale_factor; a.hf = height_factor; a.hp = height_power;
-    a.norm_mean = P[L_MEAN].as<double>();
-    a.mean_off = P[L_MOFF].as<long long>();
-    a.seq_off = P[L_SOFF].as<long long>();
-    a.read_start = P[L_START].as<long long>();
-    a.seq = P[L_SEQ].as<unsigned char>();
-    a.kmeans = ctx->model_means.as<double>();
-    a.ksds = ctx->model_sds.as<double>();
-    a.alt = ctx->alt_means.as<double>();
-    k_llr<false><<<n, 256, 0, s>>>(a, P[L_CNT].as<int>(), nullptr, nullptr, nullptr);
-    TB2_CHECK_LAUNCH(ctx);
-    std::vector<int> cnt((size_t)n);
-    TB2_CUDA_TRY(ctx, cudaMemcpyAsync(cnt.data(), P[L_CNT].p, (size_t)n * 4, cudaMemcpyDeviceToHost, s));
-    TB2_CUDA_TRY(ctx, cudaStreamSynchronize(s));
-    for (int r = 0; r < n; ++r) site_off[r + 1] = site_off[r] + cnt[r];
-    const size_t total = (size_t)site_off[n];
-    if (total == 0) return TB2_OK;
-    TB2_CUDA_TRY(ctx, P[L_LLR].reserve(total * 8));
-    TB2_CUDA_TRY(ctx, P[L_POS].reserve(total * 8));
-    TB2_CUDA_TRY(ctx, cudaMemcpyAsync(P[L_SITEOFF].p, site_off, (n + 1) * 8, cudaMemcpyHostToDevice, s));
-    k_llr<true><<<n, 256, 0, s>>>(a, nullptr, P[L_SITEOFF].as<long long>(), P[L_LLR].as<double>(),
-                                  P[L_POS].as<long long>());
-    TB2_CHECK_LAUNCH(ctx);
-    TB2_CUDA_TRY(ctx, cudaMemcpyAsync(llr_out, P[L_LLR].p, total * 8, cudaMemcpyDeviceToHost, s));
-    TB2_CUDA_TRY(ctx, cudaMemcpyAsync(pos_out, P[L_POS].p, total * 8, cudaMemcpyDeviceToHost, s));
-    TB2_CUDA_TRY(ctx, cudaStreamSynchronize(s));
-    return TB2_OK;
-}
-
-// ---------------------------------------------------------------------------
-// the same scoring on the RESIDENT batch (after tb2_batch_compute): sequence, per-base
-// means and per-read status are already in HBM, LLRs and positions stay there for
-// tb2_region_stats_add_batch_llr / tb2_batch_llr_download
-// ---------------------------------------------------------------------------
-namespace {
 // exclusive scan of the per-read site counts (one block; n is a batch, <= ~1e6)
 __global__ void __launch_bounds__(1024) k_scan_sites(const int *cnt, long long *site_off, int n)
 {
@@ -205,61 +109,169 @@ __global__ void __launch_bounds__(1024) k_scan_sites(const int *cnt, long long *
 }
 }  // namespace
 
+extern "C" int tb2_set_alt_model(tb2_ctx *ctx, const double *alt_means, int kmer_width)
+{
+    int rc = tb2_use(ctx);
+    if (rc) return rc;
+    if (!alt_means || kmer_width < 1 || kmer_width > 12) return TB2_ERR_INVALID_ARG;
+    const size_t n = ((size_t)1 << (2 * kmer_width)) * kmer_width;
+    TB2_CUDA_TRY(ctx, ctx->alt_means.upload(alt_means, n, ctx->stream));
+    TB2_CUDA_TRY(ctx, cudaStreamSynchronize(ctx->stream));
+    ctx->alt_kmer_width = kmer_width;
+    return TB2_OK;
+}
+
+namespace {
+bool alt_model_ok(tb2_ctx *ctx)
+{
+    if (ctx->kmer_width > 0 && ctx->alt_kmer_width == ctx->kmer_width) return true;
+    ctx->err = "standard and alternative models must be set with the same k-mer width";
+    return false;
+}
+
+// everything of LlrArgs but the reads
+LlrArgs llr_args(tb2_ctx *ctx, int alt_code, int use_standard_llhr, double sf, double hf, double hp)
+{
+    LlrArgs a;
+    memset(&a, 0, sizeof(a));
+    a.K = ctx->kmer_width; a.cpos = ctx->central_pos; a.alt_code = alt_code;
+    a.use_std = use_standard_llhr ? 1 : 0;
+    a.sf = sf; a.hf = hf; a.hp = hp;
+    a.kmeans = ctx->model_means.as<double>();
+    a.ksds = ctx->model_sds.as<double>();
+    a.alt = ctx->alt_means.as<double>();
+    return a;
+}
+
+// the reads of the resident batch (after tb2_batch_compute): sequence, per-base means and
+// per-read status are already in HBM; only the read starts are uploaded
+int resident_reads(tb2_ctx *ctx, const int64_t *read_start, BatchResultView *v, LlrArgs &a)
+{
+    int rc = tb2_batch_result_view(ctx, v);
+    if (rc) return rc;
+    DevBuf &start = tb2_state(ctx->llr).scratch[L_START];
+    TB2_CUDA_TRY(ctx, start.upload(read_start, (size_t)v->n_reads, ctx->stream));
+    a.n_reads = v->n_reads;
+    a.norm_mean = v->norm_mean; a.mean_off = v->base_off; a.seq_off = v->seq_off; a.seq = v->seq;
+    a.read_start = start.as<long long>();
+    a.status = v->status; a.status_stride = v->stride;
+    return TB2_OK;
+}
+
+// k_llr<FILL> or k_llr_motif<FILL>
+template <class A> using LlrKernel = void (*)(A, int *, const long long *, double *, long long *);
+
+// count -> scan -> fill over the n reads of `a`: site offsets (n + 1) into site_off, LLRs and
+// positions into llr / pos, which get room for max_sites sites.  Reads back the site count
+// and, where read_status is given, the per-read status the motif count pass wrote.
+template <class A>
+int run_llr(tb2_ctx *ctx, LlrKernel<A> count, LlrKernel<A> fill, const A &a, int n,
+            size_t max_sites, DevBuf &site_off, DevBuf &llr, DevBuf &pos, int32_t *read_status,
+            long long *total)
+{
+    auto &P = tb2_state(ctx->llr).scratch;
+    cudaStream_t s = ctx->stream;
+    TB2_CUDA_TRY(ctx, P[L_CNT].reserve((size_t)n * 4));
+    TB2_CUDA_TRY(ctx, site_off.reserve((size_t)(n + 1) * 8));
+    TB2_CUDA_TRY(ctx, llr.reserve(max_sites * 8 + 8));
+    TB2_CUDA_TRY(ctx, pos.reserve(max_sites * 8 + 8));
+    count<<<n, 256, 0, s>>>(a, P[L_CNT].as<int>(), nullptr, nullptr, nullptr);
+    TB2_CHECK_LAUNCH(ctx);
+    k_scan_sites<<<1, 1024, 0, s>>>(P[L_CNT].as<int>(), site_off.as<long long>(), n);
+    TB2_CHECK_LAUNCH(ctx);
+    fill<<<n, 256, 0, s>>>(a, nullptr, site_off.as<long long>(), llr.as<double>(), pos.as<long long>());
+    TB2_CHECK_LAUNCH(ctx);
+    TB2_CUDA_TRY(ctx, cudaMemcpyAsync(total, site_off.as<long long>() + n, 8, cudaMemcpyDeviceToHost, s));
+    if (read_status)
+        TB2_CUDA_TRY(ctx, cudaMemcpyAsync(read_status, P[L_STATUS].p, (size_t)n * 4, cudaMemcpyDeviceToHost, s));
+    TB2_CUDA_TRY(ctx, cudaStreamSynchronize(s));
+    return TB2_OK;
+}
+
+// host-array calls: sites in the per-call scratch, copied out to the caller
+template <class A>
+int run_host(tb2_ctx *ctx, LlrKernel<A> count, LlrKernel<A> fill, const A &a, int n,
+             size_t max_sites, double *llr_out, int64_t *pos_out, int64_t *site_off,
+             int32_t *read_status)
+{
+    auto &P = tb2_state(ctx->llr).scratch;
+    cudaStream_t s = ctx->stream;
+    long long total = 0;
+    int rc = run_llr(ctx, count, fill, a, n, max_sites, P[L_SITEOFF], P[L_LLR], P[L_POS],
+                     read_status, &total);
+    if (rc) return rc;
+    TB2_CUDA_TRY(ctx, cudaMemcpyAsync(site_off, P[L_SITEOFF].p, (size_t)(n + 1) * 8, cudaMemcpyDeviceToHost, s));
+    if (total) {
+        TB2_CUDA_TRY(ctx, cudaMemcpyAsync(llr_out, P[L_LLR].p, (size_t)total * 8, cudaMemcpyDeviceToHost, s));
+        TB2_CUDA_TRY(ctx, cudaMemcpyAsync(pos_out, P[L_POS].p, (size_t)total * 8, cudaMemcpyDeviceToHost, s));
+    }
+    TB2_CUDA_TRY(ctx, cudaStreamSynchronize(s));
+    return TB2_OK;
+}
+
+// resident calls: the LLRs stay in LlrState for tb2_batch_llr_download and
+// tb2_region_stats_add_batch_llr
+template <class A>
+int run_resident(tb2_ctx *ctx, LlrKernel<A> count, LlrKernel<A> fill, const A &a,
+                 const BatchResultView &v, int32_t *read_status, int64_t *n_sites_total)
+{
+    LlrState &L = tb2_state(ctx->llr);
+    long long total = 0;
+    // every site is a base: the batch's base count bounds the site count (no size round trip)
+    int rc = run_llr(ctx, count, fill, a, v.n_reads, (size_t)v.total_bases, L.site_off, L.llr,
+                     L.pos, read_status, &total);
+    if (rc) return rc;
+    L.sites = total;
+    L.reads = v.n_reads;
+    if (n_sites_total) *n_sites_total = total;
+    return TB2_OK;
+}
+}  // namespace
+
+extern "C" int tb2_alt_model_llr_batch(tb2_ctx *ctx, int64_t n_reads, const double *norm_mean,
+                                       const int64_t *mean_off, const uint8_t *seq,
+                                       const int64_t *seq_off, const int64_t *read_start,
+                                       int alt_base_code, int use_standard_llhr,
+                                       double scale_factor, double height_factor,
+                                       double height_power, double *llr_out, int64_t *pos_out,
+                                       int64_t *site_off)
+{
+    int rc = tb2_use(ctx);
+    if (rc) return rc;
+    if (!site_off || alt_base_code < 0 || alt_base_code > 3 || !alt_model_ok(ctx))
+        return TB2_ERR_INVALID_ARG;
+    LlrArgs a = llr_args(ctx, alt_base_code, use_standard_llhr, scale_factor, height_factor, height_power);
+    if ((rc = tb2_stage_reads(ctx, n_reads, norm_mean, mean_off, seq, seq_off, read_start,
+                              tb2_state(ctx->llr).scratch + L_MEAN, a)))
+        return rc;
+    const int n = a.n_reads = (int)n_reads;
+    site_off[0] = 0;
+    if (n == 0) return TB2_OK;
+    if (!norm_mean || !seq || !llr_out || !pos_out) return TB2_ERR_INVALID_ARG;
+    // every site is a base of its read: the mean count bounds the site count
+    return run_host(ctx, k_llr<false>, k_llr<true>, a, n, (size_t)mean_off[n], llr_out, pos_out,
+                    site_off, nullptr);
+}
+
 extern "C" int tb2_batch_alt_llr(tb2_ctx *ctx, const int64_t *read_start, int alt_base_code,
                                  int use_standard_llhr, double scale_factor, double height_factor,
                                  double height_power, int64_t *n_sites_total)
 {
     int rc = tb2_use(ctx);
     if (rc) return rc;
-    if (!read_start || alt_base_code < 0 || alt_base_code > 3) return TB2_ERR_INVALID_ARG;
-    if (ctx->kmer_width <= 0 || ctx->alt_kmer_width != ctx->kmer_width) {
-        ctx->err = "standard and alternative models must be set with the same k-mer width";
+    if (!read_start || alt_base_code < 0 || alt_base_code > 3 || !alt_model_ok(ctx))
         return TB2_ERR_INVALID_ARG;
-    }
+    LlrArgs a = llr_args(ctx, alt_base_code, use_standard_llhr, scale_factor, height_factor, height_power);
     BatchResultView v;
-    if ((rc = tb2_batch_result_view(ctx, &v))) return rc;
-    const int n = v.n_reads;
-    LlrState &L = tb2_state(ctx->llr);
-    auto &P = L.scratch;
-    cudaStream_t s = ctx->stream;
-    TB2_CUDA_TRY(ctx, P[L_START].reserve((size_t)n * 8));
-    TB2_CUDA_TRY(ctx, P[L_CNT].reserve((size_t)n * 4));
-    TB2_CUDA_TRY(ctx, L.site_off.reserve((size_t)(n + 1) * 8));
-    // every site is a base: the batch's base count bounds the site count (no size round trip)
-    TB2_CUDA_TRY(ctx, L.llr.reserve((size_t)v.total_bases * 8 + 8));
-    TB2_CUDA_TRY(ctx, L.pos.reserve((size_t)v.total_bases * 8 + 8));
-    TB2_CUDA_TRY(ctx, cudaMemcpyAsync(P[L_START].p, read_start, (size_t)n * 8, cudaMemcpyHostToDevice, s));
-    LlrArgs a;
-    a.n_reads = n; a.K = ctx->kmer_width; a.cpos = ctx->central_pos; a.alt_code = alt_base_code;
-    a.use_std = use_standard_llhr ? 1 : 0;
-    a.sf = scale_factor; a.hf = height_factor; a.hp = height_power;
-    a.norm_mean = v.norm_mean; a.mean_off = v.base_off; a.seq_off = v.seq_off;
-    a.read_start = P[L_START].as<long long>();
-    a.seq = v.seq;
-    a.kmeans = ctx->model_means.as<double>(); a.ksds = ctx->model_sds.as<double>();
-    a.alt = ctx->alt_means.as<double>();
-    a.status = v.status; a.status_stride = v.stride;
-    k_llr<false><<<n, 256, 0, s>>>(a, P[L_CNT].as<int>(), nullptr, nullptr, nullptr);
-    TB2_CHECK_LAUNCH(ctx);
-    k_scan_sites<<<1, 1024, 0, s>>>(P[L_CNT].as<int>(), L.site_off.as<long long>(), n);
-    TB2_CHECK_LAUNCH(ctx);
-    k_llr<true><<<n, 256, 0, s>>>(a, nullptr, L.site_off.as<long long>(), L.llr.as<double>(),
-                                  L.pos.as<long long>());
-    TB2_CHECK_LAUNCH(ctx);
-    long long total = 0;
-    TB2_CUDA_TRY(ctx, cudaMemcpyAsync(&total, L.site_off.as<long long>() + n, 8, cudaMemcpyDeviceToHost, s));
-    TB2_CUDA_TRY(ctx, cudaStreamSynchronize(s));
-    L.sites = total;
-    L.reads = n;
-    if (n_sites_total) *n_sites_total = total;
-    return TB2_OK;
+    if ((rc = resident_reads(ctx, read_start, &v, a))) return rc;
+    return run_resident(ctx, k_llr<false>, k_llr<true>, a, v, nullptr, n_sites_total);
 }
 
 // ---------------------------------------------------------------------------
 // motif models, both strands, region clipping (k_llr_motif, motif_llr.cuh)
 // ---------------------------------------------------------------------------
 namespace {
-// checks shared by both motif entry points; fills everything of `a` but the read arrays
+// checks shared by both motif entry points; fills everything of `a` but the reads and strands
 int motif_args(tb2_ctx *ctx, const tb2_motif *motif, int64_t max_motif_bb, int64_t max_motif_ab,
                int64_t reg_start, int64_t reg_end, int use_standard_llhr, double sf, double hf,
                double hp, MotifArgs *a)
@@ -271,10 +283,7 @@ int motif_args(tb2_ctx *ctx, const tb2_motif *motif, int64_t max_motif_bb, int64
         if (motif->mask[j] == 0 || motif->mask[j] > 15) return TB2_ERR_INVALID_ARG;
     if (max_motif_bb < motif->mod_pos - 1 || max_motif_ab < motif->len - motif->mod_pos)
         return TB2_ERR_INVALID_ARG;
-    if (ctx->kmer_width <= 0 || ctx->alt_kmer_width != ctx->kmer_width) {
-        ctx->err = "standard and alternative models must be set with the same k-mer width";
-        return TB2_ERR_INVALID_ARG;
-    }
+    if (!alt_model_ok(ctx)) return TB2_ERR_INVALID_ARG;
     memset(a, 0, sizeof(*a));
     a->m.len = motif->len;
     a->m.mod_pos = motif->mod_pos;
@@ -283,21 +292,21 @@ int motif_args(tb2_ctx *ctx, const tb2_motif *motif, int64_t max_motif_bb, int64
     a->max_ab = max_motif_ab;
     a->reg_start = reg_start;
     a->reg_end = reg_end;
-    LlrArgs &s = a->s;
-    s.K = ctx->kmer_width; s.cpos = ctx->central_pos; s.alt_code = -1;
-    s.use_std = use_standard_llhr ? 1 : 0;
-    s.sf = sf; s.hf = hf; s.hp = hp;
-    s.kmeans = ctx->model_means.as<double>();
-    s.ksds = ctx->model_sds.as<double>();
-    s.alt = ctx->alt_means.as<double>();
+    a->s = llr_args(ctx, -1, use_standard_llhr, sf, hf, hp);
     return TB2_OK;
 }
 
-bool strands_ok(const int8_t *strand, int n)
+// checks and uploads the strand of each of n reads; the count pass writes each read's status
+int motif_strands(tb2_ctx *ctx, int n, const int8_t *strand, MotifArgs &a)
 {
     for (int r = 0; r < n; ++r)
-        if (strand[r] < -1 || strand[r] > 1) return false;
-    return true;
+        if (strand[r] < -1 || strand[r] > 1) return TB2_ERR_INVALID_ARG;
+    auto &P = tb2_state(ctx->llr).scratch;
+    TB2_CUDA_TRY(ctx, P[L_STRAND].upload(strand, (size_t)n, ctx->stream));
+    TB2_CUDA_TRY(ctx, P[L_STATUS].reserve((size_t)n * 4));
+    a.strand = P[L_STRAND].as<signed char>();
+    a.read_status = P[L_STATUS].as<int>();
+    return TB2_OK;
 }
 }  // namespace
 
@@ -310,70 +319,21 @@ extern "C" int tb2_alt_model_llr_motif_batch(
 {
     int rc = tb2_use(ctx);
     if (rc) return rc;
-    if (n_reads < 0 || n_reads > INT_MAX || !mean_off || !seq_off || !read_start || !strand ||
-        !site_off)
-        return TB2_ERR_INVALID_ARG;
+    if (!strand || !site_off) return TB2_ERR_INVALID_ARG;
     MotifArgs a;
     if ((rc = motif_args(ctx, motif, max_motif_bb, max_motif_ab, reg_start, reg_end,
                          use_standard_llhr, scale_factor, height_factor, height_power, &a)))
         return rc;
-    const int n = (int)n_reads;
-    if (!strands_ok(strand, n)) return TB2_ERR_INVALID_ARG;
+    if ((rc = tb2_stage_reads(ctx, n_reads, norm_mean, mean_off, seq, seq_off, read_start,
+                              tb2_state(ctx->llr).scratch + L_MEAN, a.s)))
+        return rc;
+    const int n = a.s.n_reads = (int)n_reads;
+    if ((rc = motif_strands(ctx, n, strand, a))) return rc;
     site_off[0] = 0;
     if (n == 0) return TB2_OK;
     if (!norm_mean || !seq || !llr_out || !pos_out) return TB2_ERR_INVALID_ARG;
-    // every read holds nb means and the nb + K - 1 bases of their k-mers
-    for (int r = 0; r < n; ++r) {
-        const long long nb = mean_off[r + 1] - mean_off[r];
-        if (nb < 0 || nb > INT_MAX || seq_off[r + 1] - seq_off[r] != nb + (ctx->kmer_width - 1))
-            return TB2_ERR_INVALID_ARG;
-    }
-    auto &P = tb2_state(ctx->llr).scratch;
-    cudaStream_t s = ctx->stream;
-    const size_t tm = (size_t)mean_off[n], ts = (size_t)seq_off[n];
-    TB2_CUDA_TRY(ctx, P[L_MEAN].reserve(tm * 8 + 8));
-    TB2_CUDA_TRY(ctx, P[L_MOFF].reserve((n + 1) * 8));
-    TB2_CUDA_TRY(ctx, P[L_SEQ].reserve(ts + 8));
-    TB2_CUDA_TRY(ctx, P[L_SOFF].reserve((n + 1) * 8));
-    TB2_CUDA_TRY(ctx, P[L_START].reserve((size_t)n * 8));
-    TB2_CUDA_TRY(ctx, P[L_STRAND].reserve((size_t)n));
-    TB2_CUDA_TRY(ctx, P[L_STATUS].reserve((size_t)n * 4));
-    TB2_CUDA_TRY(ctx, P[L_CNT].reserve((size_t)n * 4));
-    TB2_CUDA_TRY(ctx, P[L_SITEOFF].reserve((n + 1) * 8));
-    // every site is a base of its read: the mean count bounds the site count
-    TB2_CUDA_TRY(ctx, P[L_LLR].reserve(tm * 8 + 8));
-    TB2_CUDA_TRY(ctx, P[L_POS].reserve(tm * 8 + 8));
-    TB2_CUDA_TRY(ctx, cudaMemcpyAsync(P[L_MEAN].p, norm_mean, tm * 8, cudaMemcpyHostToDevice, s));
-    TB2_CUDA_TRY(ctx, cudaMemcpyAsync(P[L_MOFF].p, mean_off, (n + 1) * 8, cudaMemcpyHostToDevice, s));
-    TB2_CUDA_TRY(ctx, cudaMemcpyAsync(P[L_SEQ].p, seq, ts, cudaMemcpyHostToDevice, s));
-    TB2_CUDA_TRY(ctx, cudaMemcpyAsync(P[L_SOFF].p, seq_off, (n + 1) * 8, cudaMemcpyHostToDevice, s));
-    TB2_CUDA_TRY(ctx, cudaMemcpyAsync(P[L_START].p, read_start, (size_t)n * 8, cudaMemcpyHostToDevice, s));
-    TB2_CUDA_TRY(ctx, cudaMemcpyAsync(P[L_STRAND].p, strand, (size_t)n, cudaMemcpyHostToDevice, s));
-    a.s.n_reads = n;
-    a.s.norm_mean = P[L_MEAN].as<double>();
-    a.s.mean_off = P[L_MOFF].as<long long>();
-    a.s.seq_off = P[L_SOFF].as<long long>();
-    a.s.read_start = P[L_START].as<long long>();
-    a.s.seq = P[L_SEQ].as<unsigned char>();
-    a.strand = P[L_STRAND].as<signed char>();
-    a.read_status = P[L_STATUS].as<int>();
-    long long *d_off = P[L_SITEOFF].as<long long>();
-    k_llr_motif<false><<<n, 256, 0, s>>>(a, P[L_CNT].as<int>(), nullptr, nullptr, nullptr);
-    TB2_CHECK_LAUNCH(ctx);
-    k_scan_sites<<<1, 1024, 0, s>>>(P[L_CNT].as<int>(), d_off, n);
-    TB2_CHECK_LAUNCH(ctx);
-    k_llr_motif<true><<<n, 256, 0, s>>>(a, nullptr, d_off, P[L_LLR].as<double>(), P[L_POS].as<long long>());
-    TB2_CHECK_LAUNCH(ctx);
-    TB2_CUDA_TRY(ctx, cudaMemcpyAsync(site_off, d_off, (size_t)(n + 1) * 8, cudaMemcpyDeviceToHost, s));
-    if (read_status)
-        TB2_CUDA_TRY(ctx, cudaMemcpyAsync(read_status, P[L_STATUS].p, (size_t)n * 4, cudaMemcpyDeviceToHost, s));
-    TB2_CUDA_TRY(ctx, cudaStreamSynchronize(s));
-    const size_t total = (size_t)site_off[n];
-    if (total == 0) return TB2_OK;
-    TB2_CUDA_TRY(ctx, cudaMemcpyAsync(llr_out, P[L_LLR].p, total * 8, cudaMemcpyDeviceToHost, s));
-    TB2_CUDA_TRY(ctx, cudaMemcpyAsync(pos_out, P[L_POS].p, total * 8, cudaMemcpyDeviceToHost, s));
-    TB2_CUDA_TRY(ctx, cudaStreamSynchronize(s));
-    return TB2_OK;
+    return run_host(ctx, k_llr_motif<false>, k_llr_motif<true>, a, n, (size_t)mean_off[n], llr_out,
+                    pos_out, site_off, read_status);
 }
 
 extern "C" int tb2_batch_alt_llr_motif(tb2_ctx *ctx, const int64_t *read_start, const int8_t *strand,
@@ -391,44 +351,9 @@ extern "C" int tb2_batch_alt_llr_motif(tb2_ctx *ctx, const int64_t *read_start, 
                          use_standard_llhr, scale_factor, height_factor, height_power, &a)))
         return rc;
     BatchResultView v;
-    if ((rc = tb2_batch_result_view(ctx, &v))) return rc;
-    const int n = v.n_reads;
-    if (!strands_ok(strand, n)) return TB2_ERR_INVALID_ARG;
-    LlrState &L = tb2_state(ctx->llr);
-    auto &P = L.scratch;
-    cudaStream_t s = ctx->stream;
-    TB2_CUDA_TRY(ctx, P[L_START].reserve((size_t)n * 8));
-    TB2_CUDA_TRY(ctx, P[L_STRAND].reserve((size_t)n));
-    TB2_CUDA_TRY(ctx, P[L_STATUS].reserve((size_t)n * 4));
-    TB2_CUDA_TRY(ctx, P[L_CNT].reserve((size_t)n * 4));
-    TB2_CUDA_TRY(ctx, L.site_off.reserve((size_t)(n + 1) * 8));
-    TB2_CUDA_TRY(ctx, L.llr.reserve((size_t)v.total_bases * 8 + 8));
-    TB2_CUDA_TRY(ctx, L.pos.reserve((size_t)v.total_bases * 8 + 8));
-    TB2_CUDA_TRY(ctx, cudaMemcpyAsync(P[L_START].p, read_start, (size_t)n * 8, cudaMemcpyHostToDevice, s));
-    TB2_CUDA_TRY(ctx, cudaMemcpyAsync(P[L_STRAND].p, strand, (size_t)n, cudaMemcpyHostToDevice, s));
-    a.s.n_reads = n;
-    a.s.norm_mean = v.norm_mean; a.s.mean_off = v.base_off; a.s.seq_off = v.seq_off;
-    a.s.read_start = P[L_START].as<long long>();
-    a.s.seq = v.seq;
-    a.s.status = v.status; a.s.status_stride = v.stride;
-    a.strand = P[L_STRAND].as<signed char>();
-    a.read_status = P[L_STATUS].as<int>();
-    k_llr_motif<false><<<n, 256, 0, s>>>(a, P[L_CNT].as<int>(), nullptr, nullptr, nullptr);
-    TB2_CHECK_LAUNCH(ctx);
-    k_scan_sites<<<1, 1024, 0, s>>>(P[L_CNT].as<int>(), L.site_off.as<long long>(), n);
-    TB2_CHECK_LAUNCH(ctx);
-    k_llr_motif<true><<<n, 256, 0, s>>>(a, nullptr, L.site_off.as<long long>(), L.llr.as<double>(),
-                                        L.pos.as<long long>());
-    TB2_CHECK_LAUNCH(ctx);
-    long long total = 0;
-    TB2_CUDA_TRY(ctx, cudaMemcpyAsync(&total, L.site_off.as<long long>() + n, 8, cudaMemcpyDeviceToHost, s));
-    if (read_status)
-        TB2_CUDA_TRY(ctx, cudaMemcpyAsync(read_status, P[L_STATUS].p, (size_t)n * 4, cudaMemcpyDeviceToHost, s));
-    TB2_CUDA_TRY(ctx, cudaStreamSynchronize(s));
-    L.sites = total;
-    L.reads = n;
-    if (n_sites_total) *n_sites_total = total;
-    return TB2_OK;
+    if ((rc = resident_reads(ctx, read_start, &v, a.s))) return rc;
+    if ((rc = motif_strands(ctx, v.n_reads, strand, a))) return rc;
+    return run_resident(ctx, k_llr_motif<false>, k_llr_motif<true>, a, v, read_status, n_sites_total);
 }
 
 extern "C" int tb2_batch_llr_download(tb2_ctx *ctx, double *llr_out, int64_t *pos_out, int64_t *site_off)
@@ -472,12 +397,10 @@ extern "C" int tb2_new_mean_stds(tb2_ctx *ctx, const double *sig, int64_t n_sig,
         if (segs[i] < 0 || segs[i] > n_sig) return TB2_ERR_INVALID_ARG;
     auto &P = tb2_state(ctx->llr).scratch;
     cudaStream_t s = ctx->stream;
-    TB2_CUDA_TRY(ctx, P[L_A].reserve((size_t)n_sig * 8));
-    TB2_CUDA_TRY(ctx, P[L_B].reserve((size_t)(n_segs + 1) * 8));
+    TB2_CUDA_TRY(ctx, P[L_A].upload(sig, (size_t)n_sig, s));
+    TB2_CUDA_TRY(ctx, P[L_B].upload(segs, (size_t)n_segs + 1, s));
     TB2_CUDA_TRY(ctx, P[L_C].reserve((size_t)n_segs * 8));
     TB2_CUDA_TRY(ctx, P[L_D].reserve((size_t)n_segs * 8));
-    TB2_CUDA_TRY(ctx, cudaMemcpyAsync(P[L_A].p, sig, (size_t)n_sig * 8, cudaMemcpyHostToDevice, s));
-    TB2_CUDA_TRY(ctx, cudaMemcpyAsync(P[L_B].p, segs, (size_t)(n_segs + 1) * 8, cudaMemcpyHostToDevice, s));
     k_mean_stds<<<(unsigned)((n_segs + 127) / 128), 128, 0, s>>>(
         P[L_A].as<double>(), P[L_B].as<long long>(), n_segs, P[L_C].as<double>(), P[L_D].as<double>());
     TB2_CHECK_LAUNCH(ctx);
@@ -552,24 +475,19 @@ extern "C" int tb2_calc_llh_ratio_windows(tb2_ctx *ctx, int mode, int64_t n_site
     if (!means || !ref_means || !alt_means || !llr_out) return TB2_ERR_INVALID_ARG;
     auto &P = tb2_state(ctx->llr).scratch;
     cudaStream_t s = ctx->stream;
-    const size_t nk = (size_t)n_sites * kmer_width * 8, nv = (size_t)n_sites * 8;
-    TB2_CUDA_TRY(ctx, P[L_MEAN].reserve(nk));
-    TB2_CUDA_TRY(ctx, P[L_A].reserve(nk));
-    TB2_CUDA_TRY(ctx, P[L_B].reserve(nk));
-    TB2_CUDA_TRY(ctx, P[L_C].reserve(mode == 2 ? nk : nv));
-    TB2_CUDA_TRY(ctx, P[L_D].reserve(mode == 2 ? nk : 8));
-    TB2_CUDA_TRY(ctx, P[L_LLR].reserve(nv));
-    TB2_CUDA_TRY(ctx, cudaMemcpyAsync(P[L_MEAN].p, means, nk, cudaMemcpyHostToDevice, s));
-    TB2_CUDA_TRY(ctx, cudaMemcpyAsync(P[L_A].p, ref_means, nk, cudaMemcpyHostToDevice, s));
-    TB2_CUDA_TRY(ctx, cudaMemcpyAsync(P[L_B].p, alt_means, nk, cudaMemcpyHostToDevice, s));
-    TB2_CUDA_TRY(ctx, cudaMemcpyAsync(P[L_C].p, var_a, mode == 2 ? nk : nv, cudaMemcpyHostToDevice, s));
-    if (mode == 2) TB2_CUDA_TRY(ctx, cudaMemcpyAsync(P[L_D].p, var_b, nk, cudaMemcpyHostToDevice, s));
+    const size_t nk = (size_t)n_sites * kmer_width, nv = (size_t)n_sites;
+    TB2_CUDA_TRY(ctx, P[L_MEAN].upload(means, nk, s));
+    TB2_CUDA_TRY(ctx, P[L_A].upload(ref_means, nk, s));
+    TB2_CUDA_TRY(ctx, P[L_B].upload(alt_means, nk, s));
+    TB2_CUDA_TRY(ctx, P[L_C].upload(var_a, mode == 2 ? nk : nv, s));
+    TB2_CUDA_TRY(ctx, P[L_D].upload(var_b, mode == 2 ? nk : 0, s));
+    TB2_CUDA_TRY(ctx, P[L_LLR].reserve(nv * 8));
     k_llh_windows<<<(unsigned)((n_sites + 127) / 128), 128, 0, s>>>(
         mode, n_sites, kmer_width, P[L_MEAN].as<double>(), P[L_A].as<double>(), P[L_B].as<double>(),
         P[L_C].as<double>(), P[L_D].as<double>(), scale_factor, height_factor, height_power,
         P[L_LLR].as<double>());
     TB2_CHECK_LAUNCH(ctx);
-    TB2_CUDA_TRY(ctx, cudaMemcpyAsync(llr_out, P[L_LLR].p, nv, cudaMemcpyDeviceToHost, s));
+    TB2_CUDA_TRY(ctx, cudaMemcpyAsync(llr_out, P[L_LLR].p, nv * 8, cudaMemcpyDeviceToHost, s));
     TB2_CUDA_TRY(ctx, cudaStreamSynchronize(s));
     return TB2_OK;
 }

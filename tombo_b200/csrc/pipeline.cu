@@ -83,10 +83,6 @@ int build_view(tb2_ctx *ctx, BatchBuffers &B, int n, const int64_t *raw_off, con
     // a stall needs > 200 consecutive observations (MEAN_STALL_PARAMS), so a read of S
     // samples holds at most S / 200 + 1 intervals: size the slots from the longest read
     const int stall_cap = (int)std::max<long long>(8, max_raw_pre / 200 + 4);
-    TB2_CUDA_TRY(ctx, B.raw_off.reserve((n + 1) * 8));
-    TB2_CUDA_TRY(ctx, B.seq_off.reserve((n + 1) * 8));
-    TB2_CUDA_TRY(ctx, B.base_off.reserve((n + 1) * 8));
-    TB2_CUDA_TRY(ctx, B.ev_off.reserve((n + 1) * 8));
     TB2_CUDA_TRY(ctx, B.seq.reserve((size_t)hb.total_seq + 8));
     TB2_CUDA_TRY(ctx, B.rawf.reserve(S * 8 + 8));
     TB2_CUDA_TRY(ctx, B.norm.reserve(S * 8 + 8));
@@ -108,10 +104,10 @@ int build_view(tb2_ctx *ctx, BatchBuffers &B, int n, const int64_t *raw_off, con
     TB2_CUDA_TRY(ctx, B.dbg.reserve((size_t)n * 3 * 4));
     TB2_CUDA_TRY(ctx, B.counters.reserve(64));
     cudaStream_t s = ctx->stream;
-    TB2_CUDA_TRY(ctx, cudaMemcpyAsync(B.raw_off.p, raw_off, (n + 1) * 8, cudaMemcpyHostToDevice, s));
-    TB2_CUDA_TRY(ctx, cudaMemcpyAsync(B.seq_off.p, seq_off, (n + 1) * 8, cudaMemcpyHostToDevice, s));
-    TB2_CUDA_TRY(ctx, cudaMemcpyAsync(B.base_off.p, hb.base_off.data(), (n + 1) * 8, cudaMemcpyHostToDevice, s));
-    TB2_CUDA_TRY(ctx, cudaMemcpyAsync(B.ev_off.p, hb.ev_off.data(), (n + 1) * 8, cudaMemcpyHostToDevice, s));
+    TB2_CUDA_TRY(ctx, B.raw_off.upload(raw_off, (size_t)n + 1, s));
+    TB2_CUDA_TRY(ctx, B.seq_off.upload(seq_off, (size_t)n + 1, s));
+    TB2_CUDA_TRY(ctx, B.base_off.upload(hb.base_off.data(), (size_t)n + 1, s));
+    TB2_CUDA_TRY(ctx, B.ev_off.upload(hb.ev_off.data(), (size_t)n + 1, s));
     // launch order: longest reads first, so that the persistent DP warps and the
     // CTA-per-read kernels do not end on a straggler (length bucketing of mixed batches)
     v.order = nullptr;
@@ -124,8 +120,7 @@ int build_view(tb2_ctx *ctx, BatchBuffers &B, int n, const int64_t *raw_off, con
             std::stable_sort(order.begin(), order.end(), [&](int a, int b) {
                 return raw_off[a + 1] - raw_off[a] > raw_off[b + 1] - raw_off[b];
             });
-            TB2_CUDA_TRY(ctx, B.order.reserve((size_t)n * 4));
-            TB2_CUDA_TRY(ctx, cudaMemcpyAsync(B.order.p, order.data(), (size_t)n * 4, cudaMemcpyHostToDevice, s));
+            TB2_CUDA_TRY(ctx, B.order.upload(order.data(), (size_t)n, s));
             TB2_CUDA_TRY(ctx, cudaStreamSynchronize(s));   // order is a local
             v.order = B.order.as<int>();
         }
@@ -316,10 +311,8 @@ extern "C" int tb2_set_model(tb2_ctx *ctx, const double *means, const double *sd
         central_pos >= kmer_width)
         return TB2_ERR_INVALID_ARG;
     const size_t n = (size_t)1 << (2 * kmer_width);
-    TB2_CUDA_TRY(ctx, ctx->model_means.reserve(n * 8));
-    TB2_CUDA_TRY(ctx, ctx->model_sds.reserve(n * 8));
-    TB2_CUDA_TRY(ctx, cudaMemcpyAsync(ctx->model_means.p, means, n * 8, cudaMemcpyHostToDevice, ctx->stream));
-    TB2_CUDA_TRY(ctx, cudaMemcpyAsync(ctx->model_sds.p, sds, n * 8, cudaMemcpyHostToDevice, ctx->stream));
+    TB2_CUDA_TRY(ctx, ctx->model_means.upload(means, n, ctx->stream));
+    TB2_CUDA_TRY(ctx, ctx->model_sds.upload(sds, n, ctx->stream));
     TB2_CUDA_TRY(ctx, cudaStreamSynchronize(ctx->stream));
     ctx->kmer_width = kmer_width;
     ctx->central_pos = central_pos;
@@ -415,8 +408,7 @@ static int batch_set_read_inputs_impl(tb2_ctx *ctx, const tb2_scale_values *sv_i
     cudaStream_t s = ctx->stream;
     h->has_sv_in = sv_in != nullptr;
     if (sv_in) {
-        TB2_CUDA_TRY(ctx, h->sv_in.reserve((size_t)n * sizeof(tb2_scale_values)));
-        TB2_CUDA_TRY(ctx, cudaMemcpyAsync(h->sv_in.p, sv_in, (size_t)n * sizeof(tb2_scale_values), cudaMemcpyHostToDevice, s));
+        TB2_CUDA_TRY(ctx, h->sv_in.upload(sv_in, (size_t)n, s));
     }
     h->has_stalls_in = stall_off != nullptr;
     if (stall_off) {
@@ -430,10 +422,8 @@ static int batch_set_read_inputs_impl(tb2_ctx *ctx, const tb2_scale_values *sv_i
                 flat[((size_t)r * cap + k) * 2 + 1] = (int)stall_ints[2 * (stall_off[r] + k) + 1];
             }
         }
-        TB2_CUDA_TRY(ctx, h->buf.stalls.reserve(flat.size() * 4 + 8));
-        TB2_CUDA_TRY(ctx, h->n_stall.reserve((size_t)n * 4));
-        TB2_CUDA_TRY(ctx, cudaMemcpyAsync(h->buf.stalls.p, flat.data(), flat.size() * 4, cudaMemcpyHostToDevice, s));
-        TB2_CUDA_TRY(ctx, cudaMemcpyAsync(h->n_stall.p, cnt.data(), (size_t)n * 4, cudaMemcpyHostToDevice, s));
+        TB2_CUDA_TRY(ctx, h->buf.stalls.upload(flat.data(), flat.size(), s));
+        TB2_CUDA_TRY(ctx, h->n_stall.upload(cnt.data(), (size_t)n, s));
         h->v.stall_ints = h->buf.stalls.as<int>();
         h->v.stall_cap = cap;
     }
@@ -801,17 +791,6 @@ int fetch_state(tb2_ctx *ctx, const BatchView &v, ReadState *st)
     TB2_CUDA_TRY(ctx, cudaMemcpyAsync(st, v.st, sizeof(ReadState), cudaMemcpyDeviceToHost, ctx->stream));
     TB2_CUDA_TRY(ctx, cudaStreamSynchronize(ctx->stream));
     return TB2_OK;
-}
-
-__global__ void k_i64_to_i32(const long long *in, int *out, long long n)
-{
-    const long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x;
-    if (i < n) out[i] = (int)in[i];
-}
-__global__ void k_i32_to_i64(const int *in, long long *out, long long n)
-{
-    const long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x;
-    if (i < n) out[i] = in[i];
 }
 
 }  // namespace

@@ -23,8 +23,10 @@
 
 namespace {
 // per-call scratch of the entry points below; nothing reads it after a call returns
+// F_MEAN .. F_START: the reads of tb2_de_novo_read_stats_batch (tb2_stage_reads; F_RM holds
+// mean_off there)
 enum { R_STAT = 0, R_POS, R_OUT_POS, R_OUT_F, R_OUT_D, R_OUT_C, R_OUT_V, R_N,
-       F_MEAN, F_RM, F_RS, F_OFF, F_OUT, F_LOGP, F_SEQ, F_SOFF, F_START, F_POS, RS_COUNT };
+       F_MEAN, F_RM, F_SEQ, F_SOFF, F_START, F_RS, F_OFF, F_OUT, F_LOGP, F_POS, RS_COUNT };
 }  // namespace
 
 struct RegionState {
@@ -142,10 +144,8 @@ extern "C" int tb2_region_stats_add(tb2_ctx *ctx, int64_t n, const double *stats
     if (n < 0 || (n > 0 && (!stats || !pos)) || isnan(single_read_thresh)) return TB2_ERR_INVALID_ARG;
     if (n == 0) return TB2_OK;
     auto &P = tb2_state(ctx->region).scratch;
-    TB2_CUDA_TRY(ctx, P[R_STAT].reserve((size_t)n * 8));
-    TB2_CUDA_TRY(ctx, P[R_POS].reserve((size_t)n * 8));
-    TB2_CUDA_TRY(ctx, cudaMemcpyAsync(P[R_STAT].p, stats, (size_t)n * 8, cudaMemcpyHostToDevice, ctx->stream));
-    TB2_CUDA_TRY(ctx, cudaMemcpyAsync(P[R_POS].p, pos, (size_t)n * 8, cudaMemcpyHostToDevice, ctx->stream));
+    TB2_CUDA_TRY(ctx, P[R_STAT].upload(stats, (size_t)n, ctx->stream));
+    TB2_CUDA_TRY(ctx, P[R_POS].upload(pos, (size_t)n, ctx->stream));
     rc = tb2_region_accumulate_dev(ctx, n, P[R_STAT].as<double>(), P[R_POS].as<long long>(),
                                    single_read_thresh, lower_thresh, stat_type);
     if (rc) return rc;
@@ -261,16 +261,11 @@ extern "C" int tb2_window_fisher_pvals(tb2_ctx *ctx, int64_t n_segs, const doubl
         return TB2_ERR_INVALID_ARG;
     auto &P = tb2_state(ctx->region).scratch;
     cudaStream_t s = ctx->stream;
-    TB2_CUDA_TRY(ctx, P[F_MEAN].reserve((size_t)total * 8 + 8));
-    TB2_CUDA_TRY(ctx, P[F_RM].reserve((size_t)total * 8 + 8));
-    TB2_CUDA_TRY(ctx, P[F_RS].reserve((size_t)total * 8 + 8));
-    TB2_CUDA_TRY(ctx, P[F_OFF].reserve((size_t)(n_segs + 1) * 8));
-    TB2_CUDA_TRY(ctx, cudaMemcpyAsync(P[F_MEAN].p, means, (size_t)total * 8, cudaMemcpyHostToDevice, s));
-    if (!is_p) {
-        TB2_CUDA_TRY(ctx, cudaMemcpyAsync(P[F_RM].p, ref_means, (size_t)total * 8, cudaMemcpyHostToDevice, s));
-        TB2_CUDA_TRY(ctx, cudaMemcpyAsync(P[F_RS].p, ref_sds, (size_t)total * 8, cudaMemcpyHostToDevice, s));
-    }
-    TB2_CUDA_TRY(ctx, cudaMemcpyAsync(P[F_OFF].p, seg_off, (size_t)(n_segs + 1) * 8, cudaMemcpyHostToDevice, s));
+    TB2_CUDA_TRY(ctx, P[F_MEAN].upload(means, (size_t)total, s));
+    // p-values in: k_fisher reads no reference levels
+    TB2_CUDA_TRY(ctx, P[F_RM].upload(ref_means, is_p ? 0 : (size_t)total, s));
+    TB2_CUDA_TRY(ctx, P[F_RS].upload(ref_sds, is_p ? 0 : (size_t)total, s));
+    TB2_CUDA_TRY(ctx, P[F_OFF].upload(seg_off, (size_t)n_segs + 1, s));
     FisherArgs a;
     memset(&a, 0, sizeof(a));
     a.means = P[F_MEAN].as<double>(); a.rm = P[F_RM].as<double>(); a.rs = P[F_RS].as<double>();
@@ -287,40 +282,23 @@ extern "C" int tb2_de_novo_read_stats_batch(tb2_ctx *ctx, int64_t n_reads, const
 {
     int rc = tb2_use(ctx);
     if (rc) return rc;
-    if (n_reads < 0 || fm_offset < 0 || fm_offset > 64 || !mean_off || !seq_off || !read_start || !stat_off)
-        return TB2_ERR_INVALID_ARG;
+    if (fm_offset < 0 || fm_offset > 64 || !stat_off) return TB2_ERR_INVALID_ARG;
     if (ctx->kmer_width <= 0) { ctx->err = "tb2_set_model has not been called"; return TB2_ERR_INVALID_ARG; }
+    auto &P = tb2_state(ctx->region).scratch;
+    FisherArgs a;
+    memset(&a, 0, sizeof(a));
+    if ((rc = tb2_stage_reads(ctx, n_reads, norm_mean, mean_off, seq, seq_off, read_start, P + F_MEAN, a)))
+        return rc;
     stat_off[0] = 0;
     if (n_reads == 0) return TB2_OK;
     const int n = (int)n_reads, K = ctx->kmer_width;
-    for (int r = 0; r < n; ++r) {
-        const long long nb = mean_off[r + 1] - mean_off[r];
-        if (nb < 0 || seq_off[r + 1] - seq_off[r] != nb + (K - 1)) return TB2_ERR_INVALID_ARG;
-        // len(r_seq) < kmer_width raises in the reference (:3846-3848): no stats for that read
-        stat_off[r + 1] = stat_off[r] + std::max<long long>(0, nb - (K - 1));
-    }
+    // len(r_seq) < kmer_width raises in the reference (:3846-3848): no stats for that read
+    for (int r = 0; r < n; ++r)
+        stat_off[r + 1] = stat_off[r] + std::max<long long>(0, mean_off[r + 1] - mean_off[r] - (K - 1));
     const long long total = stat_off[n];
     if (total > 0 && (!norm_mean || !seq || !pvals_out || !pos_out)) return TB2_ERR_INVALID_ARG;
-    auto &P = tb2_state(ctx->region).scratch;
-    cudaStream_t s = ctx->stream;
-    const size_t tm = (size_t)mean_off[n], ts = (size_t)seq_off[n];
-    TB2_CUDA_TRY(ctx, P[F_MEAN].reserve(tm * 8 + 8));
-    TB2_CUDA_TRY(ctx, P[F_RM].reserve((size_t)(n + 1) * 8));     // mean_off
-    TB2_CUDA_TRY(ctx, P[F_SEQ].reserve(ts + 8));
-    TB2_CUDA_TRY(ctx, P[F_SOFF].reserve((size_t)(n + 1) * 8));
-    TB2_CUDA_TRY(ctx, P[F_START].reserve((size_t)n * 8));
-    TB2_CUDA_TRY(ctx, P[F_OFF].reserve((size_t)(n + 1) * 8));
-    TB2_CUDA_TRY(ctx, cudaMemcpyAsync(P[F_MEAN].p, norm_mean, tm * 8, cudaMemcpyHostToDevice, s));
-    TB2_CUDA_TRY(ctx, cudaMemcpyAsync(P[F_RM].p, mean_off, (size_t)(n + 1) * 8, cudaMemcpyHostToDevice, s));
-    TB2_CUDA_TRY(ctx, cudaMemcpyAsync(P[F_SEQ].p, seq, ts, cudaMemcpyHostToDevice, s));
-    TB2_CUDA_TRY(ctx, cudaMemcpyAsync(P[F_SOFF].p, seq_off, (size_t)(n + 1) * 8, cudaMemcpyHostToDevice, s));
-    TB2_CUDA_TRY(ctx, cudaMemcpyAsync(P[F_START].p, read_start, (size_t)n * 8, cudaMemcpyHostToDevice, s));
-    TB2_CUDA_TRY(ctx, cudaMemcpyAsync(P[F_OFF].p, stat_off, (size_t)(n + 1) * 8, cudaMemcpyHostToDevice, s));
-    FisherArgs a;
-    memset(&a, 0, sizeof(a));
-    a.norm_mean = P[F_MEAN].as<double>(); a.mean_off = P[F_RM].as<long long>();
-    a.seq = P[F_SEQ].as<unsigned char>(); a.seq_off = P[F_SOFF].as<long long>();
-    a.read_start = P[F_START].as<long long>(); a.off = P[F_OFF].as<long long>();
+    TB2_CUDA_TRY(ctx, P[F_OFF].upload(stat_off, (size_t)n + 1, ctx->stream));
+    a.off = P[F_OFF].as<long long>();
     a.kmeans = ctx->model_means.as<double>(); a.ksds = ctx->model_sds.as<double>();
     a.K = K; a.cpos = ctx->central_pos;
     a.lag = (int)fm_offset; a.final_clamp = 1;

@@ -16,8 +16,7 @@ for mixed in (False, True):
     rp, sp = bench.RP(aln), bench.RP(aln, save=True)
     pol = _lib.make_policy('DNA')
     fn = ctx.lib.tb2_debug_counters
-    fn.restype = C.c_int
-    out = (C.c_uint64 * 8)()
+    out = (C.c_ulonglong * 8)()
     fn(ctx.handle, out, C.c_int(1))
     res = ctx.resquiggle_batch(raw, raw_off, seq, seq_off, rp, sp, pol)
     fn(ctx.handle, out, C.c_int(1))
