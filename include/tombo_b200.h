@@ -120,7 +120,8 @@ int64_t tb2_launch_count(tb2_ctx *ctx);
  * (banded DP, k_align), out[2] number of k_align launches, out[3] reads
  * processed summed over those launches.  After tb2_group_reg_stats / tb2_reads_ref_levels:
  * out[0] is the device time from the call's first kernel to its last (upload and download
- * excluded), out[1..3] are 0 */
+ * excluded), out[1..3] are 0.  After tb2_kernel_densities: out[0] likewise, out[1] the part
+ * of it spent in the per-set setup kernel (std, factor, kernel width), out[2..3] 0 */
 int tb2_last_timing(tb2_ctx *ctx, double *out4);
 
 /* page-locked host buffers (optional; any host memory is accepted by all calls) */
@@ -467,6 +468,26 @@ int tb2_reads_ref_levels(tb2_ctx *ctx, int64_t reg_start, int64_t reg_len, int64
                          const double *prior_sds, double mean_prior_weight,
                          double sd_prior_weight, double *means_out, double *sds_out,
                          int64_t *cov_out);
+
+/* ---- alternative-model estimation: per-k-mer Gaussian kernel densities ----------------
+ * est_kernel_density tombo_stats.py:1914-1939 for n_sets ragged sets of levels (set s is
+ * levels[off[s] .. off[s+1]), in the order parse_base_levels :1811-1884 collects them):
+ * gaussian_kde(levels, bw_method=bw / levels.std(ddof=1)).evaluate(x) on the n_points grid
+ * x.  dens_out[s * n_points + j] is the density of set s at x[j]; cho_cov_out[s] is the
+ * kernel width (scipy's cho_cov); factor_out (may be NULL) gets bw / std(ddof=1).
+ * Arithmetic (DESIGN.md §2 "Kernel densities"): std(ddof=1) and factor in numpy's pairwise
+ * order, bit-exact; cho_cov from pairwise sums where np.cov uses a BLAS dot (within
+ * gamma_n + 6u of scipy's); each term exp(-(p_i - q_j)^2 / 2) * norm times 1/n as
+ * gaussian_kernel_estimate computes it, with the device exp and a different summation
+ * order (bound in DESIGN.md).  Where the reference raises -- fewer than 2 levels, a
+ * non-finite level, zero or overflowing standard deviation -- the set's row, cho_cov and
+ * factor are NaN.  n_sets out of 0 .. 2^31 - 1, a set of more than 2^31 - 1 levels, bad
+ * offsets, n_points out of 1 .. 2^20, a NULL grid, or bw <= 0 / non-finite ->
+ * TB2_ERR_INVALID_ARG.  tb2_last_timing out[0] is the kernel time, out[1] the setup kernel's
+ * share of it. */
+int tb2_kernel_densities(tb2_ctx *ctx, int64_t n_sets, const double *levels,
+                         const int64_t *off, int64_t n_points, const double *x, double bw,
+                         double *dens_out, double *cho_cov_out, double *factor_out);
 
 #ifdef __cplusplus
 }

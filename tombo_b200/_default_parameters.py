@@ -50,3 +50,9 @@ SMALLEST_PVAL = 1e-50                      # :158
 MEAN_PRIOR_CONST = 5                       # :139
 SD_PRIOR_CONST = 40                        # :140
 COV_DAMP_COUNTS = [2, 0]                   # (unmodified, modified pseudo counts)
+ALT_EST_BATCH = 1000                       # :147
+MAX_KMER_OBS = 10000                       # :148
+MIN_KMER_OBS_TO_EST = 50                   # :149
+KERNEL_DENSITY_RANGE = (-5, 5)             # :150
+ALT_EST_PCTL = 5                           # :151
+NUM_DENS_POINTS = 500                      # :164

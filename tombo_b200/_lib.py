@@ -140,6 +140,7 @@ _PROTOS = {
                                  _I, i64, i64, i64, pI64, pF64, pI64, pI64, pI64]),
     'tb2_reads_ref_levels': (_I, [_CTX, i64, i64, i64, pF64, pI64, pI64, i64, _I, pF64, pF64, f64,
                                   f64, pF64, pF64, pI64]),
+    'tb2_kernel_densities': (_I, [_CTX, i64, pF64, pI64, i64, pF64, f64, pF64, pF64, pF64]),
 }
 
 
@@ -756,6 +757,18 @@ class Context(object):
             ptr(stat_off, i64)))
         t = int(stat_off[-1])
         return pv[:t].copy(), pos[:t].copy(), stat_off
+
+    def kernel_densities(self, levels, off, x, bw):
+        """tb2_kernel_densities -> (densities (n_sets, len(x)), cho_cov, factor).  Set s is
+        ``levels[off[s]:off[s + 1]]``; a set the reference cannot fit has NaN throughout."""
+        levels, off, x = as_f64(levels), as_i64(off), as_f64(x)
+        n = off.shape[0] - 1
+        dens = np.empty((n, x.shape[0]))
+        cho, factor = np.empty(n), np.empty(n)
+        self.check(self.lib.tb2_kernel_densities(
+            self.handle, n, ptr(levels, f64), ptr(off, i64), x.shape[0], ptr(x, f64),
+            float(bw), ptr(dens, f64), ptr(cho, f64), ptr(factor, f64)))
+        return dens, cho, factor
 
 
 def make_policy(kind='DNA', outlier_thresh=5.0, max_raw_cpts=200,

@@ -94,8 +94,10 @@ __host__ __device__ __forceinline__ int tb2_perm_index(int i, int n, uint32_t ke
 // numpy DOUBLE_pairwise_sum (np.add.reduce on contiguous float64): used by
 // np.mean in score_valid_bases / get_read_seg_score (tombo_stats.py:2338,2359).
 // Serial, executed by one thread.  The numpy routine is recursive; the recursion
-// is unrolled onto an explicit frame stack (device stacks are small).
-__device__ __forceinline__ double tb2_pairwise_leaf(const double *a, int n)
+// is unrolled onto an explicit frame stack (device stacks are small).  The one definition
+// of that order: the summands are a[0 .. n), where `a` is an array or anything with
+// a[i] and a + k (csrc/model_est.cu sums values computed on the fly).
+template <class A> __device__ __forceinline__ double tb2_pairwise_leaf(A a, int n)
 {
     if (n < 8) {
         double res = 0.;
@@ -114,7 +116,15 @@ __device__ __forceinline__ double tb2_pairwise_leaf(const double *a, int n)
     return res;
 }
 
-__device__ inline double tb2_pairwise_sum(const double *a, int n)
+// where numpy splits n > 128 summands: the size of the left part
+__host__ __device__ __forceinline__ int tb2_pairwise_split(int n)
+{
+    int n2 = n / 2;
+    n2 -= n2 % 8;
+    return n2;
+}
+
+template <class A> __device__ inline double tb2_pairwise_sum(A a, int n)
 {
     if (n <= 128) return tb2_pairwise_leaf(a, n);
     // frames: (offset, n, stage, left)
@@ -126,8 +136,7 @@ __device__ inline double tb2_pairwise_sum(const double *a, int n)
     while (sp >= 0) {
         const int fn = f_n[sp];
         if (fn <= 128) { ret = tb2_pairwise_leaf(a + f_off[sp], fn); --sp; continue; }
-        int n2 = fn / 2;
-        n2 -= n2 % 8;
+        const int n2 = tb2_pairwise_split(fn);
         if (f_stage[sp] == 0) {
             f_stage[sp] = 1;
             f_off[sp + 1] = f_off[sp]; f_n[sp + 1] = n2; f_stage[sp + 1] = 0;

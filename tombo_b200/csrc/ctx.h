@@ -56,6 +56,7 @@ struct LlrState;         // llr.cu
 struct RegionState;      // region_stats.cu
 struct GroupState;       // group_stats.cu
 struct DebugState;       // debug.cu
+struct KdeState;         // model_est.cu
 
 struct tb2_ctx {
     int device = 0;
@@ -75,6 +76,7 @@ struct tb2_ctx {
     std::shared_ptr<RegionState> region;
     std::shared_ptr<GroupState> group;
     std::shared_ptr<DebugState> debug;
+    std::shared_ptr<KdeState> kde;
     // tb2_resquiggle_batch pipelines large batches over two lanes (child contexts with
     // their own stream and buffers): H2D of chunk k+1 overlaps the kernels of chunk k
     std::vector<tb2_ctx *> lanes;
@@ -114,6 +116,22 @@ template <class T> T &tb2_state(std::shared_ptr<T> &state)
 {
     if (!state) state = std::make_shared<T>();
     return *state;
+}
+
+// tb2_last_timing after a call that recorded ev0 before its first kernel: out[0] = device ms
+// from ev0 to now (the upload before and the download after excluded); with split_at,
+// out[1] = ms from ev0 to that event (the first part of the call's kernels); the rest 0
+static inline int tb2_record_kernel_time(tb2_ctx *ctx, cudaEvent_t split_at = nullptr)
+{
+    TB2_CUDA_TRY(ctx, cudaEventRecord(ctx->ev1, ctx->stream));
+    TB2_CUDA_TRY(ctx, cudaEventSynchronize(ctx->ev1));
+    float ms = 0, first = 0;
+    TB2_CUDA_TRY(ctx, cudaEventElapsedTime(&ms, ctx->ev0, ctx->ev1));
+    if (split_at) TB2_CUDA_TRY(ctx, cudaEventElapsedTime(&first, ctx->ev0, split_at));
+    ctx->last_ms_total = ms;
+    ctx->last_ms_dp = first;
+    ctx->last_dp_launches = ctx->last_dp_reads = 0;
+    return TB2_OK;
 }
 
 static inline int tb2_use(tb2_ctx *ctx)

@@ -432,18 +432,6 @@ int gather(tb2_ctx *ctx, long long reg_start, long long reg_len, const Sample &a
     }
     return TB2_OK;
 }
-// tb2_last_timing after a level call: out[0] = device ms from the first kernel to the last
-// (the upload before and the download after excluded), out[1..3] = 0
-int record_kernel_time(tb2_ctx *ctx)
-{
-    TB2_CUDA_TRY(ctx, cudaEventRecord(ctx->ev1, ctx->stream));
-    TB2_CUDA_TRY(ctx, cudaEventSynchronize(ctx->ev1));
-    float ms = 0;
-    TB2_CUDA_TRY(ctx, cudaEventElapsedTime(&ms, ctx->ev0, ctx->ev1));
-    ctx->last_ms_total = ms;
-    ctx->last_ms_dp = ctx->last_dp_launches = ctx->last_dp_reads = 0;
-    return TB2_OK;
-}
 }  // namespace
 
 extern "C" int tb2_group_reg_stats(tb2_ctx *ctx, int64_t reg_start, int64_t reg_len,
@@ -472,7 +460,7 @@ extern "C" int tb2_group_reg_stats(tb2_ctx *ctx, int64_t reg_start, int64_t reg_
         return rc;
     const long long n = reg_len, n_pos = hdr[0], n_seg = hdr[1];
     *n_out = n_pos;
-    if (n_pos == 0) return record_kernel_time(ctx);
+    if (n_pos == 0) return tb2_record_kernel_time(ctx);
     long long *idx = P[G_IDX].as<long long>();
     const long long *offs = idx + 3 * n, *offc = offs + n + 1, *seg = offc + n + 1;
     TB2_CUDA_TRY(ctx, P[G_RES].reserve((size_t)n_pos * 3 * 8));
@@ -495,7 +483,7 @@ extern "C" int tb2_group_reg_stats(tb2_ctx *ctx, int64_t reg_start, int64_t reg_
         TB2_CHECK_LAUNCH(ctx);
         res = out;
     }
-    if ((rc = record_kernel_time(ctx))) return rc;
+    if ((rc = tb2_record_kernel_time(ctx))) return rc;
     const size_t m = (size_t)std::min<long long>(n_pos, cap);
     if (m) {
         // positions are relative to reg_start on the device
@@ -549,7 +537,7 @@ extern "C" int tb2_reads_ref_levels(tb2_ctx *ctx, int64_t reg_start, int64_t reg
     k_ref_final<<<(unsigned)((n + 255) / 256), 256, 0, q>>>(map, P[G_INT].as<int>(), n, pm, ps, mean_prior_weight,
                                                            sd_prior_weight, means, sds, cov);
     TB2_CHECK_LAUNCH(ctx);
-    if ((rc = record_kernel_time(ctx))) return rc;
+    if ((rc = tb2_record_kernel_time(ctx))) return rc;
     TB2_CUDA_TRY(ctx, cudaMemcpyAsync(means_out, means, (size_t)n * 8, cudaMemcpyDeviceToHost, q));
     TB2_CUDA_TRY(ctx, cudaMemcpyAsync(sds_out, sds, (size_t)n * 8, cudaMemcpyDeviceToHost, q));
     TB2_CUDA_TRY(ctx, cudaMemcpyAsync(cov_out, cov, (size_t)n * 8, cudaMemcpyDeviceToHost, q));

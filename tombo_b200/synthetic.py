@@ -251,3 +251,36 @@ def theil_sen_subsample(n, n_points, key):
     """Indices standing in for ``np.random.choice(n, n_points, False)``."""
     return np.array([perm_index(i, n, key) for i in range(n_points)],
                     dtype=np.int64)
+
+
+def make_event_model(kmer_width, seed=0, sd=0.2):
+    """A ``kmer_ref`` of all ``4**kmer_width`` k-mers with levels ~ N(0, 1) and one sd."""
+    rs = np.random.RandomState(seed)
+    kmers = all_kmers(kmer_width)
+    return [(km, float(m), sd) for km, m in zip(kmers, rs.normal(0.0, 1.0, len(kmers)))]
+
+
+def make_event_read(kmer_ref, central_pos, n_bases, seed, alt_base=None, alt_frac=0.0,
+                    alt_shift=0.0, noise_sd=0.15, shift=0.0):
+    """One resquiggled read as its Events columns ``(norm_mean, base)``: uniform random
+    bases; the level of base b is the model level of the k-mer centred on it (``central_pos``
+    bases before b) plus ``alt_shift`` per modified base in that k-mer, plus
+    N(0, noise_sd**2), plus ``shift`` for every base.  With ``alt_base``, each such base is modified with probability
+    ``alt_frac``.  Bases without a whole k-mer around them get the noise only."""
+    rs = np.random.RandomState(seed)
+    k = len(kmer_ref[0][0])
+    means, _ = kmer_table(kmer_ref)
+    codes = rs.randint(0, 4, n_bases)
+    mod = np.zeros(n_bases, dtype=bool)
+    if alt_base is not None:
+        mod = (codes == 'ACGT'.index(alt_base)) & (rs.uniform(size=n_bases) < alt_frac)
+    level = rs.normal(0.0, noise_sd, n_bases) + shift
+    nk = max(n_bases - k + 1, 0)
+    kidx = np.zeros(nk, dtype=np.int64)
+    n_mod = np.zeros(nk)
+    for j in range(k):
+        kidx = kidx * 4 + codes[j:j + nk]
+        n_mod += mod[j:j + nk]
+    level[central_pos:central_pos + nk] += means[kidx] + alt_shift * n_mod
+    base = np.frombuffer(codes_to_seq(codes).encode(), dtype='S1')
+    return level, base

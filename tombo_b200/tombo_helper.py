@@ -8,6 +8,7 @@ import re
 from collections import namedtuple
 
 import os
+import sys
 
 import numpy as np
 
@@ -18,7 +19,7 @@ __all__ = [
     'TomboError', 'readData', 'TomboMotif', 'resquiggleParams', 'startClipParams',
     'stallParams', 'resquiggleResults', 'alignInfo', 'genomeLocation', 'sequenceData',
     'channelInfo', 'dpResults', 'scaleValues', 'seqSampleType', 'regionStats', 'groupStats',
-    'get_seq_kmers', 'rev_comp',
+    'get_seq_kmers', 'rev_comp', 'warning_message',
     'valid_cpts_w_cap', 'valid_cpts_w_cap_t_test', 'banded_traceback',
     'adaptive_banded_forward_pass', 'get_raw_read_slot', 'get_multiple_slots_read_centric']
 
@@ -33,6 +34,12 @@ INVALID_BASE_RUNS = re.compile('[^ACGT]+')
 class TomboError(Exception):
     """tombo_helper.py:67"""
     pass
+
+
+def warning_message(message):
+    """tombo_helper.py:350-355"""
+    sys.stderr.write('*' * 20 + ' WARNING ' + '*' * 20 + '\n\t' + message + '\n')
+    sys.stderr.flush()
 
 
 def _raise_status(st):

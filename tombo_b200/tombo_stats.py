@@ -6,6 +6,10 @@ parameter loading and per-read alternative-model log-likelihood ratios
 Everything numeric runs in CUDA kernels through the C ABI (include/tombo_b200.h);
 what the reference itself does in plain Python (parameter tuples, dict look-ups,
 regex motif search, a two-line numpy score) stays plain Python here."""
+import io
+import itertools
+import re
+
 import numpy as np
 
 from . import _lib
@@ -13,7 +17,8 @@ from . import tombo_helper as th
 from ._default_parameters import (
     ALGN_PARAMS_TABLE, SEG_PARAMS_TABLE, RNA_SAMP_TYPE, DNA_SAMP_TYPE,
     MIN_EVENT_TO_SEQ_RATIO, OCLLHR_SCALE, OCLLHR_HEIGHT, OCLLHR_POWER, STALL_PARAMS,
-    FM_OFFSET_DEFAULT, SMALLEST_PVAL, MEAN_PRIOR_CONST, SD_PRIOR_CONST)
+    FM_OFFSET_DEFAULT, SMALLEST_PVAL, MEAN_PRIOR_CONST, SD_PRIOR_CONST, ALT_EST_BATCH,
+    MAX_KMER_OBS, MIN_KMER_OBS_TO_EST)
 
 __all__ = [
     'TomboModel', 'AltModel', 'normalize_raw_signal', 'compute_base_means',
@@ -23,7 +28,9 @@ __all__ = [
     'collate_reg_stats', 'calc_damp_fraction', 'calc_window_fishers_method',
     'compute_de_novo_read_stats', 'compute_sample_compare_read_stats',
     'compute_ks_tests', 'compute_u_tests', 'compute_t_tests', 'calc_window_means',
-    'compute_group_reg_stats', 'get_reads_ref', 'compute_posterior_samp_dists']
+    'compute_group_reg_stats', 'get_reads_ref', 'compute_posterior_samp_dists',
+    'parse_base_levels', 'est_kernel_density', 'write_kmer_densities_file',
+    'parse_kmer_densities_file', 'isolate_alt_density']
 
 # E|N(0,1)| = sqrt(2 / pi); the reference evaluates scipy.stats.halfnorm.expect()
 # (tombo_stats.py:84), which returns this value (SURVEY.md 8c-2)
@@ -806,3 +813,207 @@ def get_reads_ref(reg_data, min_test_reads, fm_offset, std_ref=None, prior_weigh
     if not (cov >= min_test_reads).any():
         return np.full(size, np.nan), np.full(size, np.nan), {}
     return means, sds, dict(zip(range(start, start + size), cov))
+
+
+# ---------------------------------------------------------------------------
+# alternative-model estimation (tombo_stats.py:1747-2071)
+# ---------------------------------------------------------------------------
+def _read_kmer_levels(r_data, kmer_width, central_pos):
+    """one read's k-mer codes and levels in position order, paired as
+    _parse_base_levels_worker pairs them (:1760-1772); None for a read without Events.
+    K-mers with a non-ACGT base are dropped (the reference's worker dies on them)."""
+    r_means, r_seq = th.get_multiple_slots_read_centric(
+        r_data, ['norm_mean', 'base'], r_data.corr_group)
+    if r_means is None:
+        return None
+    r_seq = b''.join(r_seq) if not isinstance(r_seq, str) else r_seq.encode()
+    codes = _BASE_CODE[np.frombuffer(r_seq, dtype=np.uint8)]
+    r_means = np.asarray(r_means, dtype=np.float64)
+    dnstrm_bases = kmer_width - central_pos - 1
+    # r_means[central_pos:-dnstrm_bases] is empty when dnstrm_bases == 0 (kept)
+    levels = r_means[central_pos:-dnstrm_bases] if dnstrm_bases > 0 else r_means[:0]
+    n = min(max(codes.shape[0] - kmer_width + 1, 0), levels.shape[0])
+    kmer = np.zeros(n, dtype=np.int64)
+    bad = np.zeros(n, dtype=bool)
+    for j in range(kmer_width):
+        c = codes[j:j + n]
+        kmer = kmer * 4 + (c & 3)
+        bad |= c > 3
+    return kmer[~bad], levels[:n][~bad]
+
+
+def parse_base_levels(all_reads, std_ref, parse_levels_batch_size, kmer_obs_thresh,
+                      max_kmer_obs, min_kmer_obs_to_est, num_processes):
+    """tombo_stats.py:1811-1884 -> ``{kmer: levels}`` for every ACGT k-mer, in
+    ``itertools.product`` order, each a float64 array.
+
+    Reads are taken in batches of ``parse_levels_batch_size``.  A k-mer that is complete
+    (more than ``max_kmer_obs`` levels) when a batch starts gets nothing from that batch;
+    every other k-mer gets all of the batch's levels, in read order, then position order --
+    the order of the reference with one process (``num_processes`` is accepted; no process
+    is started).  Parsing stops once the fewest levels among the k-mers still open exceed
+    ``kmer_obs_thresh``, or when the reads run out.  Fewer than ``min_kmer_obs_to_est``
+    levels for some k-mer raises :class:`tombo_helper.TomboError` with the reference's
+    message; fewer than ``kmer_obs_thresh`` prints its warning."""
+    kmer_width, central_pos = std_ref.kmer_width, std_ref.central_pos
+    n_kmers = 4 ** kmer_width
+    chunks = [[] for _ in range(n_kmers)]
+    totals = np.zeros(n_kmers, dtype=np.int64)
+    complete = np.zeros(n_kmers, dtype=bool)
+    reads = iter(all_reads)
+    while True:
+        batch = list(itertools.islice(reads, parse_levels_batch_size))
+        no_more_reads = len(batch) < parse_levels_batch_size
+        open_kmers = ~complete
+        if not open_kmers.any():
+            # the reference takes min() of an empty list here
+            raise th.TomboError('Every k-mer was complete before the last batch of reads; '
+                                'kmer_obs_thresh must be below max_kmer_obs.')
+        parsed = [p for p in (_read_kmer_levels(r, kmer_width, central_pos) for r in batch)
+                  if p is not None]
+        if parsed:
+            kmers = np.concatenate([k for k, _ in parsed])
+            levels = np.concatenate([lv for _, lv in parsed])
+            keep = open_kmers[kmers]
+            kmers, levels = kmers[keep], levels[keep]
+            order = np.argsort(kmers, kind='stable')
+            kmers, levels = kmers[order], levels[order]
+            bounds = np.searchsorted(kmers, np.arange(n_kmers + 1))
+            for k in np.nonzero(bounds[1:] > bounds[:-1])[0]:
+                chunks[k].append(levels[bounds[k]:bounds[k + 1]])
+            totals += bounds[1:] - bounds[:-1]
+        complete |= open_kmers & (totals > max_kmer_obs)
+        if totals[open_kmers].min() > kmer_obs_thresh or no_more_reads:
+            break
+
+    fewest_kmer_obs = int(totals.min())
+    if fewest_kmer_obs < kmer_obs_thresh:
+        if fewest_kmer_obs < min_kmer_obs_to_est:
+            raise th.TomboError(
+                'Too few minimal k-mer observations to continue to alternative estimation. '
+                'Minimal k-mer has ' + str(fewest_kmer_obs) + ' total observations and ' +
+                str(min_kmer_obs_to_est) + ' observations per k-mer are required.')
+        th.warning_message(
+            'Requested minimal k-mer observations not found in all reads. Continuing to '
+            'estimation using a k-mer with ' + str(fewest_kmer_obs) + ' total observations')
+    return dict((''.join(kmer), np.concatenate(c) if c else np.zeros(0))
+                for kmer, c in zip(itertools.product('ACGT', repeat=kmer_width), chunks))
+
+
+def write_kmer_densities_file(dens_fn, kmer_dens, save_x):
+    """tombo_stats.py:1886-1893: tab-separated ``Kmer Signal Density`` rows"""
+    rows = ('\t'.join(map(str, (kmer, x, y)))
+            for kmer, dens_i in kmer_dens.items() for x, y in zip(save_x, dens_i))
+    with io.open(dens_fn, 'wt') as fp:
+        fp.write('Kmer\tSignal\tDensity\n')
+        fp.write('\n'.join(rows) + '\n')
+
+
+def parse_kmer_densities_file(dens_fn):
+    """tombo_stats.py:1895-1912 -> ``{kmer: densities}`` in file order"""
+    kmer_dens = {}
+    with io.open(dens_fn) as fp:
+        fp.readline()
+        for line in fp:
+            kmer, _, dens_i = line.split()
+            kmer_dens.setdefault(kmer, []).append(float(dens_i))
+    if len(set(len(d) for d in kmer_dens.values())) > 1:
+        raise th.TomboError('Density file is valid.')
+    return dict((kmer, np.array(d)) for kmer, d in kmer_dens.items())
+
+
+def est_kernel_density(reads_index, std_ref, kmer_obs_thresh, density_basename, save_x,
+                       kernel_dens_bw, num_processes, alt_or_stnd_name='alt',
+                       parse_levels_batch_size=ALT_EST_BATCH, max_kmer_obs=MAX_KMER_OBS,
+                       min_kmer_obs_to_est=MIN_KMER_OBS_TO_EST, device=0):
+    """tombo_stats.py:1914-1939: shuffle the reads with numpy's global RNG (as the
+    reference does, so one seed gives one order), group their levels by k-mer
+    (:func:`parse_base_levels`), and fit every k-mer's Gaussian kernel density in one
+    device call (tb2_kernel_densities): ``gaussian_kde(levels, kernel_dens_bw /
+    levels.std(ddof=1)).evaluate(save_x)``.  Returns ``{kmer: density}`` and writes
+    ``<density_basename>.<alt_or_stnd_name>_density.txt`` when a basename is given.  A
+    k-mer whose levels the reference cannot fit raises :class:`tombo_helper.TomboError`."""
+    all_reads = list(reads_index.iter_reads())
+    np.random.shuffle(all_reads)
+    base_levels = parse_base_levels(
+        all_reads, std_ref, parse_levels_batch_size, kmer_obs_thresh, max_kmer_obs,
+        min_kmer_obs_to_est, num_processes)
+    kmers = list(base_levels)
+    off = np.concatenate([[0], np.cumsum([base_levels[k].shape[0] for k in kmers])])
+    dens, cho_cov, _ = _lib.get_context(device).kernel_densities(
+        np.concatenate([base_levels[k] for k in kmers]), off, save_x, kernel_dens_bw)
+    failed = np.nonzero(np.isnan(cho_cov))[0]
+    if failed.shape[0]:
+        raise th.TomboError(
+            'Cannot fit a kernel density to the levels of k-mer ' + kmers[failed[0]] +
+            ': fewer than 2 levels, a non-finite level or zero standard deviation.')
+    kmer_dens = dict(zip(kmers, dens))
+    if density_basename is not None:
+        write_kmer_densities_file(
+            density_basename + '.' + alt_or_stnd_name + '_density.txt', kmer_dens, save_x)
+    return kmer_dens
+
+
+def _isolate_alt_density(alt_dens, std_dens, alt_base, alt_frac_pctl, std_ref, save_x):
+    """isolate_alt_density and the discrete decisions it took: ``offsets`` {kmer: grid
+    points the alternative density moved}, ``peaks`` {kmer: (control peak, matched
+    alternative peak)} for k-mers with one ``alt_base``"""
+    save_x = np.asarray(save_x, dtype=np.float64)
+
+    def dens_mean(dens):
+        keep = dens > 1e-10
+        return np.average(save_x[keep], weights=dens[keep])
+
+    # mean shift alternative - control over the k-mers without alt_base, quadratic in the
+    # control mean
+    ctrl_means, shifts = [], []
+    for kmer in std_dens:
+        if alt_base not in kmer:
+            ctrl_means.append(dens_mean(std_dens[kmer]))
+            shifts.append(dens_mean(alt_dens[kmer]) - ctrl_means[-1])
+    offset_fit = np.poly1d(np.polyfit(ctrl_means, shifts, 2))
+    step = save_x[1] - save_x[0]
+    offsets, shifted = {}, {}
+    for kmer, dens in alt_dens.items():
+        off = int(offset_fit(dens_mean(std_dens[kmer])) / step)
+        offsets[kmer] = off
+        shifted[kmer] = (np.concatenate([np.zeros(-off), dens[:off]]) if off < 0 else
+                         np.concatenate([dens[off:], np.zeros(off)]))
+
+    peaks, ratios = {}, []
+    for kmer in std_dens:
+        if kmer.count(alt_base) != 1:
+            continue
+        ctrl, alt = std_dens[kmer], shifted[kmer]
+        ctrl_peak = np.argmax(ctrl)
+        inner = alt[1:-1]
+        alt_peaks = np.nonzero((inner > alt[:-2]) & (inner > alt[2:]))[0] + 1
+        alt_peak = alt_peaks[np.argmin(abs(alt_peaks - ctrl_peak))]
+        peaks[kmer] = (int(ctrl_peak), int(alt_peak))
+        ratios.append(alt[alt_peak] / ctrl[ctrl_peak])
+    std_frac = np.percentile(ratios, alt_frac_pctl)
+    if std_frac >= 1:
+        th.warning_message(
+            'Alternative base incorporation rate estimate is approximately 0. Consider '
+            'lowering --alt-fraction-percentile.')
+
+    model_sd = np.mean(list(std_ref.sds.values()))
+    alt_rows = []
+    for kmer in std_ref.means:
+        n_alt = kmer.count(alt_base)
+        if n_alt == 0:
+            continue
+        # the control's share of this k-mer's observations: std_frac per alt_base
+        diff_dens = shifted[kmer] - (std_dens[kmer] * std_frac**n_alt)
+        diff_dens[diff_dens < 0] = 0
+        alt_level = np.average(save_x, weights=diff_dens)
+        alt_rows.extend((kmer, m.start(), alt_level, model_sd)
+                        for m in re.finditer(alt_base, kmer))
+    alt_ref = AltModel(kmer_ref=alt_rows, central_pos=std_ref.central_pos, alt_base=alt_base)
+    return alt_ref, dict(offsets=offsets, peaks=peaks)
+
+
+def isolate_alt_density(alt_dens, std_dens, alt_base, alt_frac_pctl, std_ref, save_x):
+    """tombo_stats.py:1991-2071 (host numpy on the densities, as in the reference) ->
+    :class:`AltModel` with one row per ``alt_base`` position of each k-mer of ``std_ref``"""
+    return _isolate_alt_density(alt_dens, std_dens, alt_base, alt_frac_pctl, std_ref, save_x)[0]
