@@ -148,7 +148,8 @@ int tb2_new_mean_stds(tb2_ctx *ctx, const double *sig, int64_t n_sig,
                       double *sds_out);
 /* normalize_raw_signal tombo_stats.py:482-573 (+ c_apply_outlier_thresh
  * _c_helper.pyx:73-87).  norm_type 0 'median', 1 'median_const_scale';
- * sv_in may be NULL. */
+ * sv_in may be NULL.  With sv_in and a threshold the limits come from the median
+ * and MAD of the normalised signal, as in the reference. */
 int tb2_normalize_raw_signal(tb2_ctx *ctx, const double *raw, int64_t n,
                              int norm_type, double outlier_thresh,
                              double const_scale, const tb2_scale_values *sv_in,
@@ -278,7 +279,13 @@ int tb2_batch_upload(tb2_ctx *ctx, int64_t n_reads, const void *raw, int raw_dty
                      const tb2_policy *policy);
 /* optional, between upload and compute: per-read map_res.scale_values (sv_in[r]
  * with NaN shift = none) and map_res.stall_ints (pairs (start, end), stall_off has
- * n_reads + 1 entries counting pairs); either may be NULL */
+ * n_reads + 1 entries counting pairs, starting at 0 and never decreasing); either may
+ * be NULL, and a later call replaces both.  A changepoint c is tested against the first
+ * interval of its read, in list order, whose end is >= c (the last interval if none),
+ * as remove_stall_cpts does; any int64 interval list is accepted.  Stall inputs on an
+ * RNA-policy upload, which detects stalls itself, return TB2_ERR_INVALID_ARG; stall
+ * lists with n_reads * (longest list) above 4 * samples + 1024 pairs return
+ * TB2_ERR_CAPACITY. */
 int tb2_batch_set_read_inputs(tb2_ctx *ctx, const tb2_scale_values *sv_in,
                               const int64_t *stall_ints, const int64_t *stall_off);
 int tb2_batch_compute(tb2_ctx *ctx, const tb2_params *params,

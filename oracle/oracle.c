@@ -1209,27 +1209,43 @@ int orc_run_read(const double *raw_in, i64 n_raw, const double *rm, const double
                  uint32_t read_index, i64 *segs, double *norm_out, orc_read_result *res,
                  i64 *info)
 {
+    return orc_run_read_inputs(raw_in, n_raw, rm, rs, nb, p, save_p, pol, read_index, segs,
+                               norm_out, res, info, NULL, NULL, 0);
+}
+
+int orc_run_read_inputs(const double *raw_in, i64 n_raw, const double *rm, const double *rs,
+                        i64 nb, const orc_params *p, const orc_params *save_p,
+                        const orc_policy *pol, uint32_t read_index, i64 *segs, double *norm_out,
+                        orc_read_result *res, i64 *info, const orc_scale_values *sv_in,
+                        const i64 *stall_ints_in, i64 n_stalls_in)
+{
     double *raw = (double *)xmalloc(sizeof(double) * (size_t)(n_raw > 0 ? n_raw : 1));
     i64 *stalls = NULL, n_stalls = 0;
+    const i64 *use_stalls = stall_ints_in;
     if (pol->is_rna) {
         for (i64 i = 0; i < n_raw; i++) raw[i] = raw_in[n_raw - 1 - i];  /* :1516 */
         i64 cap = n_raw / 200 + 4;
         stalls = (i64 *)xmalloc(sizeof(i64) * 2 * (size_t)cap);
         n_stalls = orc_identify_stalls(raw, n_raw, stalls, cap);          /* :1524-1528 */
-    } else memcpy(raw, raw_in, sizeof(double) * (size_t)n_raw);
+        use_stalls = stalls;
+    } else {
+        memcpy(raw, raw_in, sizeof(double) * (size_t)n_raw);
+        n_stalls = n_stalls_in;
+    }
     uint32_t calls = 0;
     int st = ORC_OK, first_st = ORC_OK;
     i64 rescued = 0, n_iters = 0;
     for (int attempt = 0; attempt < 2; attempt++) {
         const orc_params *prm = attempt == 0 ? p : save_p;
-        st = orc_resquiggle_read(raw, n_raw, rm, rs, nb, prm, pol, NULL, 1, stalls, n_stalls,
+        /* a rescue starts again from the caller's map_res */
+        st = orc_resquiggle_read(raw, n_raw, rm, rs, nb, prm, pol, sv_in, 1, use_stalls, n_stalls,
                                  orc_subsample_key(pol->subsample_seed, read_index, calls),
                                  segs, norm_out, res);
         calls++;
         n_iters = 1;
         while (st == ORC_OK && n_iters < pol->max_scaling_iters && res->norm_params_changed) {
             orc_scale_values sv = res->sv;
-            st = orc_resquiggle_read(raw, n_raw, rm, rs, nb, prm, pol, &sv, 0, stalls, n_stalls,
+            st = orc_resquiggle_read(raw, n_raw, rm, rs, nb, prm, pol, &sv, 0, use_stalls, n_stalls,
                                      orc_subsample_key(pol->subsample_seed, read_index, calls),
                                      segs, norm_out, res);
             calls++;

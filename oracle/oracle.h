@@ -191,6 +191,15 @@ int orc_run_read(const double *raw, i64 n_raw, const double *rm,
                  const orc_params *save_p, const orc_policy *pol,
                  uint32_t read_index, i64 *segs, double *norm_out,
                  orc_read_result *res, i64 *info);
+/* orc_run_read with the caller's map_res.scale_values (sv_in, may be NULL) and, for
+ * DNA, map_res.stall_ints (n_stalls pairs, may be NULL).  The RNA policy replaces the
+ * stalls with identify_stalls, as adjust_map_res does.  orc_run_read is the NULL case. */
+int orc_run_read_inputs(const double *raw, i64 n_raw, const double *rm,
+                        const double *rs, i64 nb, const orc_params *p,
+                        const orc_params *save_p, const orc_policy *pol,
+                        uint32_t read_index, i64 *segs, double *norm_out,
+                        orc_read_result *res, i64 *info, const orc_scale_values *sv_in,
+                        const i64 *stall_ints, i64 n_stalls);
 
 uint32_t orc_subsample_key(uint32_t seed, uint32_t read_index, uint32_t call);
 i64 orc_perm_index(i64 i, i64 n, uint32_t key);

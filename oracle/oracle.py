@@ -168,6 +168,15 @@ def valid_cpts_w_cap(sig, min_base_obs, w, num_cpts, t_test=False):
     return st, out
 
 
+def remove_stall_cpts(stall_ints, cpts):
+    si, psi, nsi = _stalls_arg(stall_ints)
+    cpts, pc = _i(cpts)
+    out = np.empty(cpts.shape[0], dtype=np.int64)
+    n = lib().orc_remove_stall_cpts(psi, i64(nsi), pc, i64(cpts.shape[0]),
+                                    out.ctypes.data_as(P(i64)))
+    return out[:n].copy()
+
+
 def compute_slopes(ev, md, max_slope=1000.0):
     ev, pe = _d(ev)
     md, pm = _d(md)
@@ -345,9 +354,29 @@ def resolve_skipped_bases_with_raw(segs, rm, rs, norm, params,
     return st, out
 
 
+def _scale_values_arg(scale_values):
+    """ScaleValues struct of a 5-tuple (None -> NaN), or None"""
+    if scale_values is None:
+        return None
+    return ScaleValues(*[float('nan') if v is None else float(v) for v in scale_values])
+
+
+def _stalls_arg(stall_ints):
+    """(keep-alive array, pointer, pair count) of a stall list; None -> NULL"""
+    if stall_ints is None:
+        return None, None, 0
+    si = np.ascontiguousarray(np.asarray(stall_ints, dtype=np.int64).reshape(-1))
+    n = si.shape[0] // 2
+    if n == 0:
+        si = np.zeros(2, dtype=np.int64)
+    return si, si.ctypes.data_as(P(i64)), n
+
+
 def run_read(raw, rm, rs, params, save_params, pol, read_index=0,
-             want_norm=False):
-    """Full per-read policy (iterate + rescue).  Returns dict."""
+             want_norm=False, scale_values=None, stall_ints=None):
+    """Full per-read policy (iterate + rescue) from a map_res with the given
+    scale_values / stall_ints (None = absent; the RNA policy detects its own stalls).
+    Returns dict."""
     raw, praw = _d(raw)
     rm, pr = _d(rm); rs, ps = _d(rs)
     p, sp = params_from(params), params_from(save_params)
@@ -356,11 +385,14 @@ def run_read(raw, rm, rs, params, save_params, pol, read_index=0,
     norm = np.empty(raw.shape[0]) if want_norm else None
     res = ReadResult()
     info = np.zeros(4, dtype=np.int64)
-    st = lib().orc_run_read(
+    svi = _scale_values_arg(scale_values)
+    si, psi, nsi = _stalls_arg(stall_ints)
+    st = lib().orc_run_read_inputs(
         praw, i64(raw.shape[0]), pr, ps, i64(nb), C.byref(p), C.byref(sp),
         C.byref(pol), C.c_uint32(read_index), segs.ctypes.data_as(P(i64)),
         norm.ctypes.data_as(P(f64)) if want_norm else None, C.byref(res),
-        info.ctypes.data_as(P(i64)))
+        info.ctypes.data_as(P(i64)), C.byref(svi) if svi is not None else None,
+        psi, i64(nsi))
     out = dict(status=st, message=status_message(st), calls=int(info[0]),
                rescued=bool(info[1]), n_iters=int(info[2]),
                first_status=int(info[3]))
@@ -368,6 +400,7 @@ def run_read(raw, rm, rs, params, save_params, pol, read_index=0,
         out.update(segs=segs, read_start_rel_to_raw=res.read_start_rel_to_raw,
                    shift=res.sv.shift, scale=res.sv.scale,
                    lower_lim=res.sv.lower_lim, upper_lim=res.sv.upper_lim,
+                   outlier_thresh=res.sv.outlier_thresh,
                    sig_match_score=res.sig_match_score,
                    norm_params_changed=bool(res.norm_params_changed),
                    n_norm=res.n_norm)
@@ -385,17 +418,8 @@ def resquiggle_read(raw, rm, rs, params, pol, scale_values=None,
     segs = np.empty(nb + 1, dtype=np.int64)
     norm = np.empty(raw.shape[0])
     res = ReadResult()
-    svi = None
-    if scale_values is not None:
-        svi = ScaleValues(*[float('nan') if v is None else float(v)
-                            for v in scale_values])
-    si, psi, nsi = None, None, 0
-    if stall_ints is not None:
-        si = np.ascontiguousarray(np.asarray(stall_ints, dtype=np.int64).reshape(-1))
-        psi, nsi = si.ctypes.data_as(P(i64)), si.shape[0] // 2
-        if nsi == 0:
-            si = np.zeros(2, dtype=np.int64)
-            psi = si.ctypes.data_as(P(i64))
+    svi = _scale_values_arg(scale_values)
+    si, psi, nsi = _stalls_arg(stall_ints)
     st = lib().orc_resquiggle_read(
         praw, i64(raw.shape[0]), pr, ps, i64(nb), C.byref(p), C.byref(pol),
         C.byref(svi) if svi is not None else None, C.c_int(int(first_call)),

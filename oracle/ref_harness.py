@@ -161,9 +161,11 @@ def make_map_res(raw, genome_seq, read_id='r'):
 def run_read(raw, genome_seq, std_ref, sst, params, save_params,
              outlier_thresh=5.0, max_scaling_iters=3, key_seed=0,
              read_index=0, stable_ties=False, const_scale=None,
-             skip_seq_scaling=False):
+             skip_seq_scaling=False, scale_values=None, stall_ints=None):
     """The worker's per-read policy, restated from resquiggle.py:1492-1530 and
     1575-1595 (adjust_map_res, run_rsqgl_iters, rescue with save_params).
+    ``scale_values`` / ``stall_ints`` go into the initial map_res; for RNA,
+    adjust_map_res overwrites the stalls with identify_stalls.
 
     Returns ``(res, err, info)``: the final resquiggleResults or None, the
     TomboError/other message or None, and a dict with the call count.
@@ -173,7 +175,8 @@ def run_read(raw, genome_seq, std_ref, sst, params, save_params,
     sys.path.insert(0, REPO)
     from tombo_b200.synthetic import subsample_key
     sys.path.remove(REPO)
-    map_res = make_map_res(raw, genome_seq)
+    map_res = make_map_res(raw, genome_seq)._replace(scale_values=scale_values,
+                                                     stall_ints=stall_ints)
     info = dict(calls=0, rescued=False)
 
     def one_call(mr, prm, **kw):

@@ -171,12 +171,26 @@ def select2(values, k):
     return float(out[0]), float(out[1])
 
 
-def segment(raw, params, num_events, outlier_thresh=5.0, const_scale=None):
+def segment(raw, params, num_events, outlier_thresh=5.0, const_scale=None, scale_values=None,
+            thresh_with_sv=False, stall_ints=None):
     """k_normalize -> k_cumsum -> k_cpts -> k_event_means on one read ->
-    (status, norm, (shift, scale, lower, upper, outlier_thresh), sorted cpts, event means)"""
+    (status, norm, (shift, scale, lower, upper, outlier_thresh), sorted cpts, event means).
+    scale_values: supplied 5-tuple (None -> NaN); thresh_with_sv: winsorise them by
+    outlier_thresh (the normalize_raw_signal mirror); stall_ints: (start, end) pairs, clamped
+    to [-1, n + 1] as tb2_batch_set_read_inputs does"""
     from tombo_b200 import _lib
     L = stage_lib()
     raw = np.ascontiguousarray(raw, dtype=np.float64)
+    dp = C.POINTER(C.c_double)
+    svi = si = None
+    if scale_values is not None:
+        svi = np.array([np.nan if v is None else float(v) for v in scale_values])
+    if stall_ints is not None:
+        si = np.clip(np.asarray(stall_ints, dtype=np.int64).reshape(-1), -1, raw.shape[0] + 1)
+        si = np.ascontiguousarray(np.append(si, [0, 0]), dtype=np.int32)
+    extra = (svi.ctypes.data_as(dp) if svi is not None else None, C.c_int(int(bool(thresh_with_sv))),
+             si.ctypes.data_as(C.POINTER(C.c_int)) if si is not None else None,
+             C.c_int(0 if si is None else (si.shape[0] - 2) // 2))
     n = raw.shape[0]
     norm = np.zeros(n)
     sv = np.zeros(5)
@@ -184,12 +198,11 @@ def segment(raw, params, num_events, outlier_thresh=5.0, const_scale=None):
     em = np.zeros(num_events + 8)
     ncp, st = C.c_int(0), C.c_int(0)
     ps = _lib.params_struct(params)
-    dp = C.POINTER(C.c_double)
     L.emul_segment(raw.ctypes.data_as(dp), C.c_int(n), C.byref(ps), C.c_int(num_events),
                    C.c_double(float('nan') if outlier_thresh is None else outlier_thresh),
                    C.c_double(float('nan') if const_scale is None else const_scale),
                    norm.ctypes.data_as(dp), sv.ctypes.data_as(dp), cp.ctypes.data_as(C.POINTER(C.c_int)),
-                   C.byref(ncp), em.ctypes.data_as(dp), C.byref(st))
+                   C.byref(ncp), em.ctypes.data_as(dp), C.byref(st), *extra)
     k = ncp.value
     return st.value, norm, tuple(sv.tolist()), cp[:k].astype(np.int64), em[:max(k - 1, 0)]
 

@@ -62,10 +62,14 @@ int emul_theil_sen(const double *bm, const double *rm, int nb, double prev_shift
 
 // k_normalize -> k_cumsum / k_cpts -> k_event_means on one read (first call of
 // segment_signal resquiggle.py:1052-1117: normalize_raw_signal tombo_stats.py:482-573,
-// c_valid_cpts_w_cap(_t_test) _c_helper.pyx:89-202, c_new_means _c_helper.pyx:59-71)
+// c_valid_cpts_w_cap(_t_test) _c_helper.pyx:89-202, c_new_means _c_helper.pyx:59-71,
+// remove_stall_cpts tombo_stats.py:1576-1597).  sv_in5 (may be NULL): supplied scale values;
+// thresh_with_sv: winsorise them by outlier_thresh as tb2_normalize_raw_signal does.
+// stalls (may be NULL): n_stalls (start, end) pairs, as tb2_batch_set_read_inputs stores them.
 int emul_segment(const double *raw, int n, const tb2_params *p, int num_events, double outlier_thresh,
                  double const_scale, double *norm_out, double *sv_out5, int *cpts_out, int *n_cpts_out,
-                 double *em_out, int *status_out)
+                 double *em_out, int *status_out, const double *sv_in5, int thresh_with_sv,
+                 const int *stalls, int n_stalls)
 {
     BatchView b;
     memset(&b, 0, sizeof(b));
@@ -80,9 +84,21 @@ int emul_segment(const double *raw, int n, const tb2_params *p, int num_events, 
     b.n_reads = 1; b.max_raw = n; b.raw_off = raw_off; b.ev_off = ev_off;
     b.rawf = rawf.data(); b.norm = norm.data(); b.cs = cs.data(); b.scores = scores.data();
     b.cstate = cstate.data(); b.cpts = cpts.data(); b.em = em.data(); b.st = &st;
+    if (sv_in5) {
+        st.use_sv = 1;
+        st.sv.shift = sv_in5[0]; st.sv.scale = sv_in5[1];
+        st.sv.lower_lim = sv_in5[2]; st.sv.upper_lim = sv_in5[3]; st.sv.outlier_thresh = sv_in5[4];
+    }
+    std::vector<int> si;
+    if (stalls) {
+        si.assign(stalls, stalls + 2 * n_stalls);
+        si.resize((size_t)2 * n_stalls + 2);
+        b.stall_ints = si.data(); b.stall_cap = std::max(1, n_stalls); st.n_stalls = n_stalls;
+    }
     StagePolicy pol;
     memset(&pol, 0, sizeof(pol));
     pol.outlier_thresh = outlier_thresh; pol.const_scale = const_scale;
+    pol.thresh_with_sv = thresh_with_sv;
     emul::launch(emul::Idx3{1, 1, 1}, ST_THREADS, 0, [&]() { k_normalize(b, pol, 1); });
     if (st.status == TB2_OK) {
         if (!p->use_t_test_seg)

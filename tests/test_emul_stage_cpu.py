@@ -289,3 +289,118 @@ def test_finalize_kernel_matches_oracle(orc, dna_model, RPcls):
             bm, sig, score = emul.finalize(nsig, segs, rm, rs, shc, scc, rescale)
             assert np.array_equal(bm, want_bm) and np.array_equal(sig[:segs[-1]], want_sig[:segs[-1]])
             assert score == want_score
+
+
+def _oracle_segment_inputs(orc, raw, rp, n_ev, thresh, scale_values=None, stall_ints=None):
+    """normalize_raw_signal(raw, outlier_thresh, scale_values) -> c_valid_cpts_w_cap ->
+    remove_stall_cpts -> c_new_means on the oracle"""
+    st, norm, sv = orc.normalize_raw_signal(raw, thresh, scale_values=scale_values)
+    if st != 0:
+        return st, None, None, None, None
+    st, cp = orc.valid_cpts_w_cap(norm, rp.min_obs_per_base, rp.running_stat_width, n_ev)
+    if st != 0:
+        return st, norm, sv, None, None
+    cp = np.sort(cp)
+    if stall_ints is not None:
+        cp = orc.remove_stall_cpts(stall_ints, cp)
+    return 0, norm, sv, cp, orc.new_means(norm, cp)
+
+
+def _same(a, b):
+    return all(x == y or (np.isnan(x) and np.isnan(y)) for x, y in zip(a, b))
+
+
+@pytest.mark.parametrize('odd', [True, False])
+@pytest.mark.parametrize('integer', [False, True])
+def test_normalize_supplied_scale_values_with_threshold(orc, dna_model, RPcls, odd, integer):
+    """normalize_raw_signal(raw, outlier_thresh=t, scale_values=sv) recomputes the winsorising
+    limits from the median and MAD of the normalised signal (tombo_stats.py:558-563).  k_normalize
+    in the mirror mode must do the same for odd and even n, continuous and integer-valued signal,
+    supplied values with finite and with None limits, t = 5 and t = 0.5; None limits without a
+    threshold leave the signal unclipped"""
+    import emul
+    from read_inputs_cases import NORM_THRESHOLDS, norm_scale_values
+    from tombo_b200 import synthetic as syn
+    kmer_ref, cpos = dna_model
+    rp = RPcls(seg=(5, 3, 1, 5))
+    raw = np.asarray(syn.make_read(kmer_ref, cpos, 300, 4343).raw, dtype=np.float64)
+    if integer:
+        raw = np.round(raw)
+    if (len(raw) & 1) != odd:
+        raw = raw[:-1]
+    n_ev = max(raw.shape[0] // rp.mean_obs_per_event, 330)
+    cases = [(name, sv, t) for name, sv in norm_scale_values(raw) for t in NORM_THRESHOLDS]
+    cases.append(('shifted_none', norm_scale_values(raw)[1][1], None))
+    for name, sv_in, t in cases:
+        so, onorm, osv, ocp, oem = _oracle_segment_inputs(orc, raw, rp, n_ev, t, scale_values=sv_in)
+        se, norm, sv, cp, em = emul.segment(raw, rp, n_ev, outlier_thresh=t, scale_values=sv_in,
+                                            thresh_with_sv=True)
+        assert so == se == 0, (name, t, so, se)
+        assert _same(sv, osv), (name, t, sv, osv)
+        assert np.array_equal(norm, onorm), (name, t)
+        assert np.array_equal(cp, ocp) and np.array_equal(em, oem), (name, t)
+
+
+def test_segment_with_supplied_scale_values_keeps_their_limits(orc, dna_model, RPcls):
+    """the resquiggle path (segment_signal) never winsorises supplied scale values by a
+    threshold: without the mirror flag k_normalize clips to the supplied limits"""
+    import emul
+    from read_inputs_cases import norm_scale_values
+    from tombo_b200 import synthetic as syn
+    kmer_ref, cpos = dna_model
+    rp = RPcls(seg=(5, 3, 1, 5))
+    raw = np.asarray(syn.make_read(kmer_ref, cpos, 300, 4344).raw, dtype=np.float64)
+    n_ev = max(raw.shape[0] // rp.mean_obs_per_event, 330)
+    for name, sv_in in norm_scale_values(raw):
+        so, onorm, osv, ocp, oem = _oracle_segment_inputs(orc, raw, rp, n_ev, None, scale_values=sv_in)
+        se, norm, sv, cp, em = emul.segment(raw, rp, n_ev, outlier_thresh=5.0, scale_values=sv_in)
+        assert so == se == 0
+        assert _same(sv, osv), (name, sv, osv)
+        assert np.array_equal(norm, onorm) and np.array_equal(cp, ocp), name
+
+
+def test_remove_stall_cpts_restatement_matches_oracle(orc):
+    """the oracle's remove_stall_cpts is the reference's iterator walk, on every list shape"""
+    from read_inputs_cases import remove_stall_cpts, stall_lists
+    rs = np.random.RandomState(3)
+    for it in range(20):
+        n = int(rs.randint(800, 5000))
+        cpts = np.sort(rs.choice(np.arange(1, n), size=n // 8, replace=False))
+        lists = stall_lists(n, cpts)
+        lists['random'] = [tuple(sorted(rs.randint(-5, n + 5, size=2))) for _ in range(rs.randint(1, 6))]
+        lists['random_unordered'] = [tuple(rs.randint(-5, n + 5, size=2)) for _ in range(rs.randint(1, 6))]
+        for name, si in lists.items():
+            assert np.array_equal(orc.remove_stall_cpts(si, cpts), remove_stall_cpts(si, cpts)), (it, name)
+
+
+@pytest.mark.parametrize('shape', ['planted', 'sorted', 'unsorted', 'overlapping', 'nested_inner_first',
+                                   'nested_outer_first', 'endpoints', 'empty', 'huge'])
+def test_segment_stall_removal_matches_oracle(orc, dna_model, RPcls, shape):
+    """k_cpts drops a changepoint as remove_stall_cpts does: tested only against the first
+    interval, in list order, whose end is >= it (the last if none).  Unsorted, overlapping and
+    nested lists are where 'inside any interval' differs; endpoints equal to changepoints check
+    that both comparisons are strict; +-2^40 checks the clamp to the signal's range"""
+    import emul
+    from read_inputs_cases import remove_stall_cpts, stall_lists
+    from tombo_b200 import synthetic as syn
+    kmer_ref, cpos = dna_model
+    rp = RPcls(seg=(5, 3, 1, 5))
+    stall = (150, 1500) if shape == 'planted' else None
+    raw = np.asarray(syn.make_read(kmer_ref, cpos, 400, 4545, stall=stall).raw, dtype=np.float64)
+    n_ev = max(raw.shape[0] // rp.mean_obs_per_event, 440)
+    so, onorm, osv, ocp, oem = _oracle_segment_inputs(orc, raw, rp, n_ev, 5.0)
+    assert so == 0
+    if shape == 'planted':
+        si = [tuple(int(v) for v in iv) for iv in orc.identify_stalls(raw)]
+        assert len(si) >= 1
+    else:
+        si = stall_lists(raw.shape[0], ocp)[shape]
+    want = remove_stall_cpts(si, ocp)
+    so, onorm, osv, ocp2, oem = _oracle_segment_inputs(orc, raw, rp, n_ev, 5.0, stall_ints=si)
+    assert np.array_equal(ocp2, want)
+    if shape not in ('empty',):
+        assert len(want) < len(ocp)
+    se, norm, sv, cp, em = emul.segment(raw, rp, n_ev, outlier_thresh=5.0, stall_ints=si)
+    assert se == 0
+    assert np.array_equal(cp, want), (shape, len(cp), len(want))
+    assert np.array_equal(em, oem)

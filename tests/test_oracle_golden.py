@@ -82,3 +82,54 @@ def test_subsampler_matches_python_definition(orc):
             assert lib.orc_perm_index(C.c_int64(i), C.c_int64(n), C.c_uint32(key)) == idx[i]
     assert lib.orc_subsample_key(C.c_uint32(3), C.c_uint32(7), C.c_uint32(2)) == \
         syn.subsample_key(3, 7, 2)
+
+
+def test_oracle_normalize_with_scale_values_matches_reference():
+    """normalize_raw_signal(raw, outlier_thresh, scale_values) as the reference returned it
+    (tests/golden/rsqgl_inputs.npz): signal and all five values, None <-> NaN"""
+    import oracle as orc
+    import read_inputs_cases as ric
+    for raw, t, sv, want_norm, want in ric.golden_norm_cases(ric.golden()):
+        st, norm, out = orc.normalize_raw_signal(raw, outlier_thresh=t, scale_values=sv)
+        assert st == 0
+        assert np.array_equal(norm, want_norm), (len(raw), t, sv)
+        assert all((w is None and np.isnan(o)) or o == w for o, w in zip(out, want)), (out, want)
+
+
+def test_oracle_read_inputs_match_reference(orc, RPcls):
+    """resquiggle_read with caller scale values / stall lists (single calls, orc_resquiggle_read)
+    and the worker policy from such a map_res (orc_run_read_inputs) against the reference"""
+    import read_inputs_cases as ric
+    cases = ric.golden_cases(ric.golden(), RPcls)
+    for i, c in enumerate(cases):
+        rm, rsd = gu.levels(c['read'].genome_seq, c['kmer_ref'])
+        raw = np.asarray(c['read'].raw, dtype=np.float64)
+        e = c['expected']
+        if c['call'] == 0:
+            pol = orc.policy('DNA', skip_seq_scaling=c['skip'], const_scale=c['const_scale'])
+            o = orc.resquiggle_read(raw, rm, rsd, c['rp'], pol, scale_values=c['scale_values'],
+                                    stall_ints=c['stall_ints'])
+            sv = o.get('scale_values')
+        else:
+            o = orc.run_read(raw, rm, rsd, c['rp'], c['sp'], orc.policy(c['kind']),
+                             read_index=c['read_index'], scale_values=c['scale_values'],
+                             stall_ints=c['stall_ints'])
+            assert (o['calls'], o['rescued']) == (e['calls'], e['rescued']), i
+            sv = None if o['status'] else tuple(o[k] for k in ('shift', 'scale', 'lower_lim',
+                                                               'upper_lim', 'outlier_thresh'))
+        if e['message']:
+            assert ric.same_message(o['status'], o['message'], e['message']), (i, o['message'])
+            continue
+        assert o['status'] == 0, (i, o['message'])
+        assert np.array_equal(o['segs'], e['segs']), i
+        assert o['read_start_rel_to_raw'] == e['read_start_rel_to_raw'], i
+        assert all((w is None and np.isnan(v)) or v == w for v, w in zip(sv, e['scale_values'])), \
+            (i, sv, e['scale_values'])
+        assert o['sig_match_score'] == e['sig_match_score'], i
+        assert o['norm_params_changed'] == e['norm_params_changed'], i
+        if c['call'] == 1:
+            assert o['n_iters'] == e['n_iters'], i
+    # what the cases are there for
+    worker_sv = [c for c in cases if c['call'] == 1 and c['scale_values'] is not None and c['kind'] == 'DNA']
+    assert any(c['expected']['rescued'] for c in worker_sv), 'no read with scale values rescued'
+    assert any(c['expected']['message'] for c in cases), 'no failing case'

@@ -32,6 +32,12 @@ def test_normalize_bit_exact(ctx, orc, seed, n):
     assert s0 == s1 == 0
     assert np.array_equal(n0, n1)
     assert sv0b[:4] == sv1b[:4]
+    # provided scale values and a threshold: limits from the normalised signal's median / MAD
+    s0, n0, sv0t = orc.normalize_raw_signal(raw, outlier_thresh=2.5, scale_values=sv_in)
+    s1, n1, sv1t = ctx.normalize_raw_signal(raw, outlier_thresh=2.5, scale_values=sv_in)
+    assert s0 == s1 == 0
+    assert np.array_equal(n0, n1)
+    assert sv0t == sv1t
     # no winsorising
     s0, n0, _ = orc.normalize_raw_signal(raw)
     s1, n1, _ = ctx.normalize_raw_signal(raw)

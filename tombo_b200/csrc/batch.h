@@ -75,6 +75,7 @@ struct StagePolicy {
     unsigned int subsample_seed;
     int literal_key;             // mirror API: subsample_seed already is the key
     int read_index_base;         // index of the batch's first read in the caller's batch
+    int thresh_with_sv;          // mirror API: winsorise supplied scale values by outlier_thresh
 };
 
 // launch wrappers (stage_kernels.cu); all enqueue on ctx->stream

@@ -241,6 +241,7 @@ StagePolicy stage_policy(const tb2_policy &pl)
     sp.subsample_seed = pl.subsample_seed;
     sp.literal_key = 0;
     sp.read_index_base = 0;
+    sp.thresh_with_sv = 0;
     return sp;
 }
 
@@ -328,6 +329,7 @@ struct BatchHolder {
     BatchView v;
     std::vector<int64_t> raw_off;
     int raw_dtype = 0;
+    bool is_rna = false;
     bool uploaded = false, computed = false, has_norm_sig = false;
     bool has_sv_in = false, has_stalls_in = false;
     BatchBuffers buf;                  // behind v
@@ -378,6 +380,7 @@ static int batch_upload_impl(tb2_ctx *ctx, int64_t n_reads, const void *raw, int
     if (rc) return rc;
     h->raw_off.assign(raw_off, raw_off + n + 1);
     h->raw_dtype = raw_dtype;
+    h->is_rna = policy->is_rna != 0;
     cudaStream_t s = ctx->stream;
     const size_t esz = raw_dtype == 0 ? 8 : 2;
     TB2_CUDA_TRY(ctx, h->raw_in.reserve((size_t)h->hb.total_s * esz + 8));
@@ -406,27 +409,47 @@ static int batch_set_read_inputs_impl(tb2_ctx *ctx, const tb2_scale_values *sv_i
     if (!h->uploaded) { ctx->err = "tb2_batch_upload has not been called"; return TB2_ERR_INVALID_ARG; }
     const int n = h->hb.n;
     cudaStream_t s = ctx->stream;
+    int cap = 1;
+    if (stall_off) {
+        // the RNA worker policy detects stalls itself (adjust_map_res, resquiggle.py:1524-1528)
+        if (h->is_rna) { ctx->err = "stall inputs are not taken by an RNA-policy upload"; return TB2_ERR_INVALID_ARG; }
+        if (stall_off[0] != 0) { ctx->err = "stall_off[0] is not 0"; return TB2_ERR_INVALID_ARG; }
+        for (int r = 0; r < n; ++r) {
+            const int64_t c = stall_off[r + 1] - stall_off[r];
+            if (c < 0 || c > 0x3fffffff) { ctx->err = "stall_off decreases or a read holds more than 2^30 stalls"; return TB2_ERR_INVALID_ARG; }
+            cap = std::max<int>(cap, (int)c);
+        }
+        if (stall_off[n] > 0 && !stall_ints) { ctx->err = "stall_ints is NULL"; return TB2_ERR_INVALID_ARG; }
+        // the device holds cap pairs per read: bound that padded layout (a few times the
+        // samples of the batch is far more than any stall list needs)
+        if ((double)n * cap > 4.0 * (double)h->hb.total_s + 1024.0) {
+            ctx->err = "stall lists: n_reads * (longest list) exceeds 4 * samples + 1024 pairs";
+            return TB2_ERR_CAPACITY;
+        }
+    }
     h->has_sv_in = sv_in != nullptr;
     if (sv_in) {
         TB2_CUDA_TRY(ctx, h->sv_in.upload(sv_in, (size_t)n, s));
     }
     h->has_stalls_in = stall_off != nullptr;
     if (stall_off) {
-        int cap = 1;
-        for (int r = 0; r < n; ++r) cap = std::max<int>(cap, (int)(stall_off[r + 1] - stall_off[r]));
+        // changepoints lie in [1, max_raw - 1]: clamping to [-1, max_raw + 1] keeps every
+        // comparison of remove_stall_cpts, so any int64 value gives the reference's result
+        const int64_t lo = -1, hi = (int64_t)h->v.max_raw + 1;
+        auto clamp = [&](int64_t x) { return (int)std::min(hi, std::max(lo, x)); };
         std::vector<int> flat((size_t)n * 2 * cap, 0), cnt((size_t)n, 0);
         for (int r = 0; r < n; ++r) {
             cnt[r] = (int)(stall_off[r + 1] - stall_off[r]);
             for (int k = 0; k < cnt[r]; ++k) {
-                flat[((size_t)r * cap + k) * 2] = (int)stall_ints[2 * (stall_off[r] + k)];
-                flat[((size_t)r * cap + k) * 2 + 1] = (int)stall_ints[2 * (stall_off[r] + k) + 1];
+                flat[((size_t)r * cap + k) * 2] = clamp(stall_ints[2 * (stall_off[r] + k)]);
+                flat[((size_t)r * cap + k) * 2 + 1] = clamp(stall_ints[2 * (stall_off[r] + k) + 1]);
             }
         }
         TB2_CUDA_TRY(ctx, h->buf.stalls.upload(flat.data(), flat.size(), s));
         TB2_CUDA_TRY(ctx, h->n_stall.upload(cnt.data(), (size_t)n, s));
-        h->v.stall_ints = h->buf.stalls.as<int>();
         h->v.stall_cap = cap;
     }
+    if (!h->is_rna) h->v.stall_ints = stall_off ? h->buf.stalls.as<int>() : nullptr;
     TB2_CUDA_TRY(ctx, cudaStreamSynchronize(s));
     return TB2_OK;
 }
@@ -812,11 +835,11 @@ extern "C" int tb2_normalize_raw_signal(tb2_ctx *ctx, const double *raw, int64_t
     memset(&sp, 0, sizeof(sp));
     sp.outlier_thresh = outlier_thresh;
     sp.const_scale = norm_type == 1 ? const_scale : NAN;
+    sp.thresh_with_sv = 1;
     if ((rc = tb2_launch_normalize(ctx, o.v, sp, 1))) return rc;
     TB2_CUDA_TRY(ctx, cudaMemcpyAsync(norm_out, o.v.norm, (size_t)n * 8, cudaMemcpyDeviceToHost, ctx->stream));
     if ((rc = fetch_state(ctx, o.v, &st))) return rc;
     *sv_out = st.sv;
-    if (sv_in == nullptr) sv_out->outlier_thresh = outlier_thresh;
     return st.status;
 }
 

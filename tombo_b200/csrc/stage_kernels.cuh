@@ -162,10 +162,12 @@ k_normalize(BatchView b, StagePolicy pol, int first_call)
     }
     for (int i = threadIdx.x; i < n; i += ST_THREADS) norm[i] = (raw[i] - shift) / scale;  // :554
     __syncthreads();
-    const double thresh = given ? NAN : pol.outlier_thresh;
+    // the resquiggle path never passes a threshold with scale values (segment_signal);
+    // normalize_raw_signal(outlier_thresh=t, scale_values=sv) does (thresh_with_sv)
+    const double thresh = (given && !pol.thresh_with_sv) ? NAN : pol.outlier_thresh;
     if (!isnan(thresh)) {                                                             // :559-563
         double med, mad;
-        if ((n & 1) && !use_const) {
+        if ((n & 1) && !use_const && !given) {
             // odd n: shift is an element of raw and scale an element of |raw - shift|.
             // x -> (x - shift) / scale is monotone (each rounding is), so the middle
             // order statistic of norm is the image of shift: (shift - shift) / scale = +0;
@@ -174,8 +176,9 @@ k_normalize(BatchView b, StagePolicy pol, int first_call)
             med = 0.0;
             mad = 1.0;
         } else {
-            // even n: the two middle elements of norm are the images of raw's
-            if (n & 1) med = tb2_block_median([&](int i) { return norm[i]; }, n, sm);
+            // even n with raw's own shift: the two middle elements of norm are the images
+            // of raw's; supplied shift / scale need not be raw's medians, so select on norm
+            if ((n & 1) || given) med = tb2_block_median([&](int i) { return norm[i]; }, n, sm);
             else med = (((mid_a - shift) / scale) + ((mid_b - shift) / scale)) / 2.0;
             mad = tb2_block_median([&](int i) { return fabs(norm[i] - med); }, n, sm);
         }
@@ -428,6 +431,11 @@ k_cpts(BatchView b, tb2_params p, int on_raw, int smem_words)
     }
     if (N > 1 && (int)higher + 1 >= bound) { if (tid == 0) s.status = TB2_ERR_FEWER_CPTS; return; }
     // ---- ordered compaction (+ w), dropping changepoints inside stalls ----
+    // remove_stall_cpts walks the intervals in list order alongside the ascending
+    // changepoints and tests c only against the first interval whose end is >= c (the
+    // last one if none is).  Every interval the walk passed before reaching c ends
+    // before an earlier changepoint, hence before c, so that interval depends on c
+    // alone and each candidate is decided on its own.
     const int *si = b.stall_ints ? b.stall_ints + 2 * (size_t)b.stall_cap * r : nullptr;
     const int ns = b.stall_ints ? s.n_stalls : 0;
     for (int wd = warp; wd < nw; wd += ST_THREADS / 32) {
@@ -437,7 +445,11 @@ k_cpts(BatchView b, tb2_params p, int on_raw, int smem_words)
             const double v = sc[i];
             keep = v > vN || (v == vN && i >= posN);
             const int c = i + w;
-            for (int k = 0; keep && k < ns; ++k) if (si[2 * k] < c && c < si[2 * k + 1]) keep = false;
+            if (keep && ns > 0) {
+                int k = 0;
+                while (k + 1 < ns && c > si[2 * k + 1]) ++k;
+                if (si[2 * k] < c && c < si[2 * k + 1]) keep = false;
+            }
         }
         const uint32_t kw = __ballot_sync(TB2_FULL_MASK, keep);
         if (lane == 0) K[wd] = kw;

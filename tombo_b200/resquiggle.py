@@ -239,14 +239,16 @@ def _run_batch(map_results, std_ref, rsqgl_params, save_params, outlier_thresh, 
         a, b = res['seg_off'][i], res['seg_off'][i + 1]
         segs = res['segs'][a:b].copy()
         svr = res['scale_values'][i]
+        none = lambda v: None if np.isnan(v) else float(v)   # noqa: E731
         ro = raw_off[i]
         out.append(mr._replace(
             read_start_rel_to_raw=int(res['read_start_rel_to_raw'][i]), segs=segs,
             genome_seq=mr.genome_seq[cpos:cpos + (b - a - 1)],
             raw_signal=res['norm_signal'][ro:ro + int(segs[-1])].copy(),
-            scale_values=th.scaleValues(
-                float(svr[0]), float(svr[1]), None if np.isnan(svr[2]) else float(svr[2]),
-                None if np.isnan(svr[3]) else float(svr[3]), outlier_thresh),
+            # outlier_thresh is None where the reference keeps normalize_raw_signal's value:
+            # supplied scale values or RNA event scaling without sequence rescaling
+            scale_values=th.scaleValues(float(svr[0]), float(svr[1]), none(svr[2]),
+                                        none(svr[3]), none(svr[4])),
             sig_match_score=float(res['sig_match_score'][i]),
             norm_params_changed=bool(res['flags'][i] & 1)))
     return out
