@@ -161,11 +161,14 @@ def make_map_res(raw, genome_seq, read_id='r'):
 def run_read(raw, genome_seq, std_ref, sst, params, save_params,
              outlier_thresh=5.0, max_scaling_iters=3, key_seed=0,
              read_index=0, stable_ties=False, const_scale=None,
-             skip_seq_scaling=False, scale_values=None, stall_ints=None):
+             skip_seq_scaling=False, scale_values=None, stall_ints=None,
+             max_raw_cpts=None, min_event_to_seq_ratio=None):
     """The worker's per-read policy, restated from resquiggle.py:1492-1530 and
     1575-1595 (adjust_map_res, run_rsqgl_iters, rescue with save_params).
     ``scale_values`` / ``stall_ints`` go into the initial map_res; for RNA,
-    adjust_map_res overwrites the stalls with identify_stalls.
+    adjust_map_res overwrites the stalls with identify_stalls.  ``max_raw_cpts`` and
+    ``min_event_to_seq_ratio`` are passed to every resquiggle_read call when given
+    (None: the reference's defaults).
 
     Returns ``(res, err, info)``: the final resquiggleResults or None, the
     TomboError/other message or None, and a dict with the call count.
@@ -178,10 +181,16 @@ def run_read(raw, genome_seq, std_ref, sst, params, save_params,
     map_res = make_map_res(raw, genome_seq)._replace(scale_values=scale_values,
                                                      stall_ints=stall_ints)
     info = dict(calls=0, rescued=False)
+    call_kw = {}
+    if max_raw_cpts is not None:
+        call_kw['max_raw_cpts'] = max_raw_cpts
+    if min_event_to_seq_ratio is not None:
+        call_kw['min_event_to_seq_ratio'] = min_event_to_seq_ratio
 
     def one_call(mr, prm, **kw):
         key = subsample_key(key_seed, read_index, info['calls'])
         info['calls'] += 1
+        kw.update(call_kw)
         with keyed_choice(key):
             return rsq.resquiggle_read(mr, std_ref, prm, outlier_thresh,
                                        seq_samp_type=sst, **kw)

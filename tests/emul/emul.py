@@ -31,6 +31,9 @@ def lib():
         _LIB.emul_tb_words.restype = C.c_size_t
         _LIB.emul_tb_words.argtypes = [C.c_longlong] * 3
         _LIB.emul_row_cells.argtypes = [C.c_longlong]
+        _LIB.emul_abs_chunk.argtypes = [C.c_longlong]
+        _LIB.emul_abs_ms_chunk.argtypes = [C.c_longlong]
+        _LIB.emul_wpl_of.argtypes = [C.c_int]
     return _LIB
 
 

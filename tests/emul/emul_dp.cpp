@@ -49,6 +49,11 @@ int emul_align_batch(int klass, int n_reads, const int *cpts, const double *em,
 
 size_t emul_tb_words(long long rows, long long W, long long drift) { return tb2_tb_words(rows, W, drift); }
 int emul_row_cells(long long W) { return tb2_row_cells(W); }
+// the adaptive-band engine choice of the device source (kernels.h, dp_align.cuh), for the
+// tests that place parameter points on either side of each boundary
+int emul_abs_chunk(long long W) { return tb2_abs_chunk_host(W); }
+int emul_abs_ms_chunk(long long W) { return tb2_abs_ms_chunk_host(W); }
+int emul_wpl_of(int chunk) { return tb2_wpl_of(chunk); }
 }
 
 // tuning counters of the adaptive engines (meaningful when built with -DTB2_DP_COUNTERS)

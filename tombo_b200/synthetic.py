@@ -35,9 +35,13 @@ def all_kmers(k):
     return [''.join(p) for p in itertools.product('ACGT', repeat=k)]
 
 
-def make_kmer_ref(kind='DNA', seed=0):
+def make_kmer_ref(kind='DNA', seed=0, sd_range=None):
     """Return ``(kmer_ref, central_pos)`` with ``kmer_ref`` a list of
-    ``(kmer, mean, sd)`` tuples suitable for ``TomboModel(kmer_ref=...)``."""
+    ``(kmer, mean, sd)`` tuples suitable for ``TomboModel(kmer_ref=...)``.
+
+    ``sd_range=(lo, hi)`` gives every k-mer its own sd, uniform on [lo, hi) and drawn after
+    the levels (so the levels are those of the one-sd model of the same seed), as real
+    models have; by default every k-mer has the kind's one sd."""
     rs = np.random.RandomState(seed)
     if kind == 'DNA':
         k, cpos, sd = DNA_KMER, DNA_CENTRAL, 0.2
@@ -47,7 +51,10 @@ def make_kmer_ref(kind='DNA', seed=0):
         raise ValueError(kind)
     kmers = all_kmers(k)
     means = rs.normal(0.0, 1.4826, len(kmers))
-    return [(km, float(m), sd) for km, m in zip(kmers, means)], cpos
+    if sd_range is None:
+        return [(km, float(m), sd) for km, m in zip(kmers, means)], cpos
+    sds = rs.uniform(float(sd_range[0]), float(sd_range[1]), len(kmers))
+    return [(km, float(m), float(s)) for km, m, s in zip(kmers, means, sds)], cpos
 
 
 def make_alt_kmer_ref(kmer_ref, alt_base='C', seed=1, delta_sd=0.3):
