@@ -528,8 +528,21 @@ __device__ long long tb2_wf_total_words(const int *starts, int r_end, int W)
     return __any_sync(TB2_FULL_MASK, bad) ? -1 : sum;
 }
 
-// shifted z-score of one cell for the wavefront engine.  The divide is the exact
-// reciprocal form (tb2_div_by): inv_sd = tb2_rcp_of(sd) once per row.
+// shifted z-score of one cell for the wavefront engine, from its event mean m (not read
+// for a masked cell).  The divide is the exact reciprocal form (tb2_div_by): inv_sd =
+// tb2_rcp_of(sd) once per row.
+template <int MODE, bool WIN>
+__device__ __forceinline__ double tb2_wf_z_of(double m, int j, double mu, double sd,
+                                              tb2_rcp inv_sd, int lo, int hi, double maskval,
+                                              double zs, double mhz)
+{
+    if (MODE == TB2_MODE_MASKED && (j < lo || j >= hi)) return maskval;
+    double a = tb2_div_by(fabs(m - mu), sd, inv_sd);
+    if (WIN) a = (mhz < a) ? mhz : a;
+    return zs - a;
+}
+
+// the same with the event mean (or the explicit z-score) read here
 template <int MODE, bool WIN>
 __device__ __forceinline__ double tb2_wf_z(const double *ep, int j, double mu, double sd,
                                            tb2_rcp inv_sd, int lo, int hi, double maskval,
@@ -537,9 +550,7 @@ __device__ __forceinline__ double tb2_wf_z(const double *ep, int j, double mu, d
 {
     if (MODE == TB2_MODE_EXPLICIT) return zrow[j];
     if (MODE == TB2_MODE_MASKED && (j < lo || j >= hi)) return maskval;
-    double a = tb2_div_by(fabs(__ldg(ep) - mu), sd, inv_sd);
-    if (WIN) a = (mhz < a) ? mhz : a;
-    return zs - a;
+    return tb2_wf_z_of<MODE, WIN>(__ldg(ep), j, mu, sd, inv_sd, lo, hi, maskval, zs, mhz);
 }
 
 // strip-chaining row buffer: shared-memory accesses when it lives in shared memory
@@ -573,6 +584,22 @@ __device__ __forceinline__ void tb2_rb_st(double *rb, unsigned rb_s, int i, doub
 // written at step U by lane s - U alone, read by lane s - U + 1 at step U + 1 and
 // overwritten by lane s - U - 1 later in that same step: one __syncwarp() after the load
 // and one after the store order the three (each compiles to a NOP in this converged loop).
+//
+// The event means are software-pipelined TB2_WF_MD = 3 steps deep: step U reads the mean of
+// step U + 3 into m2 and turns the mean of step U + 1, which is already in m1, into the
+// z-score of step U + 1, so that chain does not depend on step U's recurrence.  Every cell
+// gets the z-score tb2_wf_z would give it, with the same operations in the same order.  At 64
+// registers ptxas still schedules each load 16-32 instructions ahead of its first use (7-10
+// without the pipeline) and the z-score chain next to the recurrence that consumes it.
+// Loads that fall into the next group read from epn, which is ep + 16 when that group runs
+// and ep (this group's own first steps, whose means are then simply not used) when it does
+// not, and a masked row loads only unmasked cells: no address outside what the loop reads is
+// touched, and no predicate stays live across the group.
+#define TB2_WF_MD 3
+#define TB2_WF_MLD(m, K)                                                                        \
+    if (MODE != TB2_MODE_MASKED ||                                                              \
+        (unsigned)(((K) < 16 ? j + (K) : j + nadv + (K) - 16) - lo) < (unsigned)(hi - lo))      \
+        m = __ldg(((K) < 16 ? ep : epn) + ((K) < 16 ? (K) : (K) - 16));
 #ifdef TB2_EMUL
 #define TB2_WF_PLD(up, U) if (l0flag) up = tb2_lds(rd_a + 8 * (U));
 #else
@@ -582,14 +609,17 @@ __device__ __forceinline__ void tb2_rb_st(double *rb, unsigned rb_s, int i, doub
 #endif
 #define TB2_WF_FAST_STEP(U)                                                                     \
     {                                                                                           \
+        const double mz = m1;                       /* mean of step U + 1 (arrived)  */       \
+        m1 = m2;                                    /* mean of step U + 2 (in flight) */       \
+        TB2_WF_MLD(m2, (U) + TB2_WF_MD)             /* mean of step U + 3             */       \
         double up;                                                                              \
         if ((U) == 0) {                                                                         \
             up = __shfl_up_sync(TB2_FULL_MASK, xout, 1);                                        \
             TB2_WF_PLD(up, U)                                                                   \
         } else up = tb2_lds(rd_a + 8u * (U));                                                   \
         __syncwarp();                                                                           \
-        const double zn = tb2_wf_z<MODE, WIN>(ep + (U) + 1, j + (U) + 1, mu, sd, inv_sd, lo,    \
-                                              hi, maskval, nullptr, zs, mhz);                   \
+        const double zn = tb2_wf_z_of<MODE, WIN>(mz, j + (U) + 1, mu, sd, inv_sd, lo, hi,       \
+                                                 maskval, zs, mhz);                             \
         const double a = (x - stay) + z;                                                        \
         double cc = up_prev + z;                                                                \
         const double sk = up - skip;                                                            \
@@ -771,8 +801,14 @@ __device__ __noinline__ int tb2_wavefront_rows_t(const PassCtx &pc, const DpCons
         }
         if (lean && t + 15 <= t_hi) {
             // ---------- steady state: groups of 16 steps, no band-edge predicates, z one
-            // step ahead, one coalesced move-word store per group ----------
+            // step ahead and event means TB2_WF_MD steps ahead, one coalesced move-word
+            // store per group ----------
             double z = tb2_wf_z<MODE, WIN>(ep, j, mu, sd, inv_sd, lo, hi, maskval, nullptr, zs, mhz);
+            int nadv = 0;                        // the prologue stays inside the first group
+            const double *epn = ep;
+            double m1 = 0.0, m2 = 0.0;
+            TB2_WF_MLD(m1, 1)
+            TB2_WF_MLD(m2, 2)
             // lane 0 loads along the chaining row (cell above), the tail lane stores along
             // it (own cell); everyone else goes through the ring
             unsigned rd_a = lane == 0 ? rb_s + 8u * (unsigned)(j + d) : ring_s + 8u * (unsigned)(lane - 2);
@@ -781,6 +817,8 @@ __device__ __noinline__ int tb2_wavefront_rows_t(const PassCtx &pc, const DpCons
             const unsigned l0flag = lane == 0;
             uint32_t *tbp = tbs + ((t - t_begin) >> 4) * 32 + lane;
             for (; t + 15 <= t_hi; t += 16) {
+                nadv = t + 31 <= t_hi ? 16 : 0;  // the next group runs: prefetch into it
+                epn = ep + nadv;
                 TB2_WF_FAST_STEP(0) TB2_WF_FAST_STEP(1) TB2_WF_FAST_STEP(2) TB2_WF_FAST_STEP(3)
                 TB2_WF_FAST_STEP(4) TB2_WF_FAST_STEP(5) TB2_WF_FAST_STEP(6) TB2_WF_FAST_STEP(7)
                 TB2_WF_FAST_STEP(8) TB2_WF_FAST_STEP(9) TB2_WF_FAST_STEP(10) TB2_WF_FAST_STEP(11)
@@ -816,6 +854,8 @@ __device__ __noinline__ int tb2_wavefront_rows_t(const PassCtx &pc, const DpCons
     return TB2_OK;
 }
 #undef TB2_WF_FAST_STEP
+#undef TB2_WF_MLD
+#undef TB2_WF_MD
 
 __device__ int tb2_wavefront_rows(const PassCtx &pc, const DpConsts &c, int mode, int r_end,
                                   double *rowbuf, uint32_t *tbw, int *argmax_out)
