@@ -118,7 +118,8 @@ int64_t tb2_launch_count(tb2_ctx *ctx);
 /* device time (ms, CUDA events on the ctx stream) of the last tb2_batch_compute:
  * out[0] whole compute stage, out[1] sum over launches of the dominant kernel
  * (banded DP, k_align), out[2] number of k_align launches, out[3] reads
- * processed summed over those launches.  After tb2_group_reg_stats / tb2_reads_ref_levels:
+ * processed summed over those launches.  After tb2_group_reg_stats / tb2_reads_ref_levels /
+ * tb2_kmer_level_summaries / tb2_kmer_medians:
  * out[0] is the device time from the call's first kernel to its last (upload and download
  * excluded), out[1..3] are 0.  After tb2_kernel_densities: out[0] likewise, out[1] the part
  * of it spent in the per-set setup kernel (std, factor, kernel width), out[2..3] 0 */
@@ -495,6 +496,31 @@ int tb2_reads_ref_levels(tb2_ctx *ctx, int64_t reg_start, int64_t reg_len, int64
 int tb2_kernel_densities(tb2_ctx *ctx, int64_t n_sets, const double *levels,
                          const int64_t *off, int64_t n_points, const double *x, double bw,
                          double *dens_out, double *cho_cov_out, double *factor_out);
+
+/* ---- standard and motif k-mer model estimation ------------------------------------------
+ * Per-position level summaries of get_region_kmer_levels tombo_stats.py:1263-1280 and
+ * 1349-1355 for a batch of regions laid end to end in positions 0 .. n_pos - 1.  Reads are
+ * ragged genome-ordered levels (read r is levels[off[r] .. off[r+1]) starting at position
+ * start[r]; levels outside 0 .. n_pos - 1 are ignored).  cov_out[p] is the number of
+ * non-NaN levels at p.  Where cov_out[p] > cov_thresh: level_out[p], sd_out[p] are
+ * calc_med_sd (:1236-1240: np.median, np.std) or, with est_mean, c_mean_std
+ * (_c_helper.pyx:22-36) of the levels in read order; elsewhere NaN.  Arithmetic: DESIGN.md
+ * §2 "K-mer model estimation".  n_pos out of 1 .. 2^24, more than 2^30 - 1 reads, bad
+ * offsets, cov_thresh out of 0 .. 2^31 - 2 or a NULL output -> TB2_ERR_INVALID_ARG.
+ * tb2_last_timing out[0] is the kernel time. */
+int tb2_kmer_level_summaries(tb2_ctx *ctx, int64_t n_pos, int64_t n_reads, const double *levels,
+                             const int64_t *off, const int64_t *start, int64_t cov_thresh,
+                             int est_mean, double *level_out, double *sd_out, int64_t *cov_out);
+/* Grouped medians of tabulate_kmer_levels :1462-1487 and tabulate_mod_kmer_levels
+ * :2116-2144: for each key k in 0 .. n_keys - 1, count_out[k] observations i with
+ * keys[i] == k, and np.median of their levels and of their sds (the mean of the two middle
+ * values for an even count; NaN for no observation), exact.  The key is the base-4 k-mer
+ * code, or code * kmer_width + offset for motif k-mers.  n_keys out of 1 .. 2^24, n_obs out
+ * of 0 .. 2^30, a key out of range, a NaN level or sd, or a NULL pointer ->
+ * TB2_ERR_INVALID_ARG.  tb2_last_timing out[0] is the kernel time. */
+int tb2_kmer_medians(tb2_ctx *ctx, int64_t n_keys, int64_t n_obs, const int64_t *keys,
+                     const double *levels, const double *sds, int64_t *count_out,
+                     double *level_med_out, double *sd_med_out);
 
 #ifdef __cplusplus
 }

@@ -56,3 +56,4 @@ MIN_KMER_OBS_TO_EST = 50                   # :149
 KERNEL_DENSITY_RANGE = (-5, 5)             # :150
 ALT_EST_PCTL = 5                           # :151
 NUM_DENS_POINTS = 500                      # :164
+NUM_READS_TO_ADJUST_MODEL = 5000           # :174

@@ -141,6 +141,8 @@ _PROTOS = {
     'tb2_reads_ref_levels': (_I, [_CTX, i64, i64, i64, pF64, pI64, pI64, i64, _I, pF64, pF64, f64,
                                   f64, pF64, pF64, pI64]),
     'tb2_kernel_densities': (_I, [_CTX, i64, pF64, pI64, i64, pF64, f64, pF64, pF64, pF64]),
+    'tb2_kmer_level_summaries': (_I, [_CTX, i64, i64, pF64, pI64, pI64, i64, _I, pF64, pF64, pI64]),
+    'tb2_kmer_medians': (_I, [_CTX, i64, i64, pI64, pF64, pF64, pI64, pF64, pF64]),
 }
 
 
@@ -769,6 +771,31 @@ class Context(object):
             self.handle, n, ptr(levels, f64), ptr(off, i64), x.shape[0], ptr(x, f64),
             float(bw), ptr(dens, f64), ptr(cho, f64), ptr(factor, f64)))
         return dens, cho, factor
+
+    def kmer_level_summaries(self, n_pos, reads, cov_thresh, est_mean=False):
+        """tb2_kmer_level_summaries -> (levels, sds, cov), each n_pos long.  ``reads`` are
+        ragged genome-ordered reads ``(levels, off, start)`` in positions 0 .. n_pos - 1;
+        levels and sds are NaN where the coverage is not above ``cov_thresh``."""
+        lv, off, st = as_f64(reads[0]), as_i64(reads[1]), as_i64(reads[2])
+        n = int(n_pos)
+        levels, sds, cov = np.empty(n), np.empty(n), np.empty(n, dtype=np.int64)
+        self.check(self.lib.tb2_kmer_level_summaries(
+            self.handle, n, off.shape[0] - 1, ptr(lv, f64), ptr(off, i64), ptr(st, i64),
+            int(cov_thresh), int(bool(est_mean)), ptr(levels, f64), ptr(sds, f64), ptr(cov, i64)))
+        return levels, sds, cov
+
+    def kmer_medians(self, n_keys, keys, levels, sds):
+        """tb2_kmer_medians -> (counts, median levels, median sds), each n_keys long (NaN
+        medians for a key without observations)"""
+        keys, levels, sds = as_i64(keys), as_f64(levels), as_f64(sds)
+        if not keys.shape[0] == levels.shape[0] == sds.shape[0]:
+            raise ValueError('keys, levels and sds must have one entry per observation')
+        n = int(n_keys)
+        cnt, med_lv, med_sd = np.empty(n, dtype=np.int64), np.empty(n), np.empty(n)
+        self.check(self.lib.tb2_kmer_medians(
+            self.handle, n, keys.shape[0], ptr(keys, i64), ptr(levels, f64), ptr(sds, f64),
+            ptr(cnt, i64), ptr(med_lv, f64), ptr(med_sd, f64)))
+        return cnt, med_lv, med_sd
 
 
 def make_policy(kind='DNA', outlier_thresh=5.0, max_raw_cpts=200,

@@ -57,6 +57,7 @@ struct RegionState;      // region_stats.cu
 struct GroupState;       // group_stats.cu
 struct DebugState;       // debug.cu
 struct KdeState;         // model_est.cu
+struct KmerModelState;   // kmer_model.cu
 
 struct tb2_ctx {
     int device = 0;
@@ -77,6 +78,7 @@ struct tb2_ctx {
     std::shared_ptr<GroupState> group;
     std::shared_ptr<DebugState> debug;
     std::shared_ptr<KdeState> kde;
+    std::shared_ptr<KmerModelState> kmer;
     // tb2_resquiggle_batch pipelines large batches over two lanes (child contexts with
     // their own stream and buffers): H2D of chunk k+1 overlaps the kernels of chunk k
     std::vector<tb2_ctx *> lanes;

@@ -291,3 +291,49 @@ def make_event_read(kmer_ref, central_pos, n_bases, seed, alt_base=None, alt_fra
     level[central_pos:central_pos + nk] += means[kidx] + alt_shift * n_mod
     base = np.frombuffer(codes_to_seq(codes).encode(), dtype='S1')
     return level, base
+
+
+MappedRead = namedtuple('MappedRead', (
+    'start', 'end', 'strand', 'fn', 'corr_group', 'rna', 'read_start_rel_to_raw', 'chrm'))
+
+
+def make_mapped_reads(kmer_ref, central_pos, genome_len, n_reads, read_len, seed, chrm='chr',
+                      noise_sd=0.15, obs_per_base=6, rna=False):
+    """Genome-mapped resquiggled reads on both strands for model estimation.
+
+    Returns ``(genome, reads, served)``: a uniform random genome, ``MappedRead`` rows
+    (``start``/``end``/``strand``; lengths ``read_len`` +- 20 %, clipped to the genome) and
+    ``served[fn]`` = the read's columns: ``norm_mean`` and ``base`` in read order (reverse
+    complement for ``-``), ``start`` (event starts in the raw signal) and ``Signal`` (raw
+    samples: ``obs_per_base`` per base at the base's level, read order, reversed for RNA).
+    A base's level is the model level of the k-mer centred on it in read order plus
+    N(0, noise_sd**2); bases without a whole k-mer get the noise only."""
+    rs = np.random.RandomState(seed)
+    k = len(kmer_ref[0][0])
+    means, _ = kmer_table(kmer_ref)
+    genome = codes_to_seq(rs.randint(0, 4, genome_len))
+    reads, served = [], {}
+    for i in range(n_reads):
+        n = int(read_len * rs.uniform(0.8, 1.2))
+        start = int(rs.randint(0, max(genome_len - n, 1)))
+        end = min(start + n, genome_len)
+        strand = '+-'[rs.randint(2)]
+        seq = genome[start:end]
+        if strand == '-':
+            seq = seq.translate(str.maketrans('ACGT', 'TGCA'))[::-1]
+        codes = seq_to_codes(seq).astype(np.int64)
+        nb = codes.shape[0]
+        level = rs.normal(0.0, noise_sd, nb)
+        nk = max(nb - k + 1, 0)
+        kidx = np.zeros(nk, dtype=np.int64)
+        for j in range(k):
+            kidx = kidx * 4 + codes[j:j + nk]
+        level[central_pos:central_pos + nk] += means[kidx]
+        ev_start = np.arange(nb, dtype=np.int64) * obs_per_base
+        sig = np.repeat(level, obs_per_base) + rs.normal(0.0, 0.05, nb * obs_per_base)
+        fn = '%s_read%d' % (chrm, i)
+        served[fn] = dict(norm_mean=level, base=np.frombuffer(seq.encode(), dtype='S1'),
+                          start=ev_start.astype(np.uint32),
+                          Signal=(sig[::-1] if rna else sig) * 80.0 + 400.0)
+        reads.append(MappedRead(start, end, strand, fn, 'RawGenomeCorrected_000', rna, 0, chrm))
+    return genome, reads, served

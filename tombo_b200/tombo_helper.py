@@ -19,7 +19,7 @@ __all__ = [
     'TomboError', 'readData', 'TomboMotif', 'resquiggleParams', 'startClipParams',
     'stallParams', 'resquiggleResults', 'alignInfo', 'genomeLocation', 'sequenceData',
     'channelInfo', 'dpResults', 'scaleValues', 'seqSampleType', 'regionStats', 'groupStats',
-    'get_seq_kmers', 'rev_comp', 'warning_message',
+    'get_seq_kmers', 'rev_comp', 'warning_message', 'parse_locs_file',
     'valid_cpts_w_cap', 'valid_cpts_w_cap_t_test', 'banded_traceback',
     'adaptive_banded_forward_pass', 'get_raw_read_slot', 'get_multiple_slots_read_centric']
 
@@ -182,6 +182,79 @@ class TomboMotif(object):
             self.mod_base = raw_motif[mod_pos - 1]
             if INVALID_BASES.match(self.mod_base):
                 raise TomboError('Modified base within motif must be a single base.')
+            self._compute_partial_patterns()
+
+    def _compute_partial_patterns(self):
+        """tombo_helper.py:565-592: patterns of the partial matches that hold mod_pos, keyed
+        by 'start' / 'end' / 'short' and the partial length"""
+        self._partial_pats = {'start': {}, 'end': {}, 'short': {}}
+        for offset in range(self.mod_pos - 1):
+            self._partial_pats['start'][self.motif_len - offset - 1] = (
+                self._parse_motif(self.raw_motif[offset + 1:]), self.mod_pos - offset - 1)
+        for offset in range(self.motif_len - self.mod_pos):
+            self._partial_pats['end'][self.motif_len - offset - 1] = (
+                self._parse_motif(self.raw_motif[:-(offset + 1)]), self.mod_pos)
+        for short_len in range(1, self.motif_len):
+            self._partial_pats['short'][short_len] = [
+                (self._parse_motif(self.raw_motif[offset:offset + short_len]), self.mod_pos - offset)
+                for offset in range(max(0, self.mod_pos - short_len),
+                                    min(self.motif_len - short_len + 1, self.mod_pos))]
+
+    def _partial_hits(self, seq):
+        """the 1-based mod positions of every full or partial match in ``seq``, in the order
+        matches_seq / find_mod_poss (:637-707) test them"""
+        for start_len in range(1, min(len(seq) + 1, self.motif_len)):
+            if start_len in self._partial_pats['start']:
+                pat, mod_pos = self._partial_pats['start'][start_len]
+                if pat.match(seq[:start_len]):
+                    yield mod_pos
+        if len(seq) < self.motif_len:
+            for pat, mod_pos in self._partial_pats['short'][len(seq)]:
+                if pat.match(seq):
+                    yield mod_pos
+        else:
+            for m in self.motif_pat.finditer(seq):
+                yield m.start() + self.mod_pos
+        for end_len in range(1, min(len(seq) + 1, self.motif_len)):
+            if end_len in self._partial_pats['end']:
+                pat, mod_pos = self._partial_pats['end'][end_len]
+                if pat.match(seq[-end_len:]):
+                    yield len(seq) - end_len + mod_pos
+
+    def matches_seq(self, seq):
+        """tombo_helper.py:637-670: does a full or partial match hold mod_pos in ``seq``"""
+        return any(True for _ in self._partial_hits(seq))
+
+    def find_mod_poss(self, seq):
+        """tombo_helper.py:672-707: sorted 1-based mod positions of the full and partial
+        matches in ``seq``"""
+        return sorted(set(self._partial_hits(seq)))
+
+
+def parse_locs_file(locs_fn):
+    """tombo_helper.py:475-506: BED single-base locations -> ``{(chrm, strand): sorted
+    positions}``; badly formatted lines are counted and warned about"""
+    n_added, n_failed = 0, 0
+    raw_locs = {}
+    with open(locs_fn) as locs_fp:
+        for line in locs_fp:
+            try:
+                chrm, pos, _, _, _, strand = line.split()[:6]
+                pos = int(pos)
+                raw_locs.setdefault((chrm, strand), set()).add(pos)
+                n_added += 1
+            except Exception:
+                n_failed += 1
+    if n_failed > 0:
+        if n_added > 0:
+            warning_message((
+                'Some provided locations ({}) were incorrectly formatted. ' +
+                'Ensure that provided file ({}) is in BED format.').format(n_failed, locs_fn))
+        else:
+            warning_message((
+                'All provided locations from {} were incorrectly formatted. ' +
+                'Ensure that provided file is in BED format.').format(locs_fn))
+    return dict((cs, np.array(sorted(cs_poss))) for cs, cs_poss in raw_locs.items())
 
 
 # ---- native wrappers (tombo_helper.py:76-102) -> CUDA -----------------------------

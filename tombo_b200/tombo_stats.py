@@ -18,7 +18,8 @@ from ._default_parameters import (
     ALGN_PARAMS_TABLE, SEG_PARAMS_TABLE, RNA_SAMP_TYPE, DNA_SAMP_TYPE,
     MIN_EVENT_TO_SEQ_RATIO, OCLLHR_SCALE, OCLLHR_HEIGHT, OCLLHR_POWER, STALL_PARAMS,
     FM_OFFSET_DEFAULT, SMALLEST_PVAL, MEAN_PRIOR_CONST, SD_PRIOR_CONST, ALT_EST_BATCH,
-    MAX_KMER_OBS, MIN_KMER_OBS_TO_EST)
+    MAX_KMER_OBS, MIN_KMER_OBS_TO_EST, NUM_READS_TO_ADJUST_MODEL, COLLAPSE_RNA_STALLS,
+    USE_RNA_EVENT_SCALE, OUTLIER_THRESH)
 
 __all__ = [
     'TomboModel', 'AltModel', 'normalize_raw_signal', 'compute_base_means',
@@ -30,7 +31,9 @@ __all__ = [
     'compute_ks_tests', 'compute_u_tests', 'compute_t_tests', 'calc_window_means',
     'compute_group_reg_stats', 'get_reads_ref', 'compute_posterior_samp_dists',
     'parse_base_levels', 'est_kernel_density', 'write_kmer_densities_file',
-    'parse_kmer_densities_file', 'isolate_alt_density']
+    'parse_kmer_densities_file', 'isolate_alt_density', 'extract_kmer_levels',
+    'tabulate_kmer_levels', 'tabulate_mod_kmer_levels', 'center_model_to_median_norm',
+    'estimate_kmer_model', 'estimate_motif_alt_model']
 
 # E|N(0,1)| = sqrt(2 / pi); the reference evaluates scipy.stats.halfnorm.expect()
 # (tombo_stats.py:84), which returns this value (SURVEY.md 8c-2)
@@ -116,6 +119,18 @@ class TomboModel(object):
             raise th.TomboError('Invalid sequence encountered from genome sequence.')
         return ref_means, ref_sds
 
+    def _center_model(self, shift_corr_factor, scale_corr_factor):
+        """tombo_stats.py:587-595"""
+        self.means = dict((kmer, (k_mean * scale_corr_factor) + shift_corr_factor)
+                          for kmer, k_mean in self.means.items())
+        self._tables = None
+
+    def _make_constant_sd(self):
+        """tombo_stats.py:597-600"""
+        med_sd = np.median(list(self.sds.values()))
+        self.sds = dict((kmer, med_sd) for kmer in self.sds)
+        self._tables = None
+
     def get_exp_levels_from_seq_with_gaps(self, reg_seq, rev_strand):
         """tombo_stats.py:886-918: expected levels of every k-mer of ``reg_seq``; NaN for
         k-mers that touch a non-ACGT base"""
@@ -173,6 +188,11 @@ class AltModel(object):
                 t[_kmer_code(k), pos] = v
             self._table = t
         return self._table
+
+    def _make_constant_sd(self):
+        """tombo_stats.py:955-958"""
+        med_sd = np.median(list(self.sds.values()))
+        self.sds = dict((kmer, med_sd) for kmer in self.sds)
 
     def get_exp_level(self, kmer, pos):
         return self.means.get((kmer, pos), np.nan)
@@ -1017,3 +1037,434 @@ def isolate_alt_density(alt_dens, std_dens, alt_base, alt_frac_pctl, std_ref, sa
     """tombo_stats.py:1991-2071 (host numpy on the densities, as in the reference) ->
     :class:`AltModel` with one row per ``alt_base`` position of each k-mer of ``std_ref``"""
     return _isolate_alt_density(alt_dens, std_dens, alt_base, alt_frac_pctl, std_ref, save_x)[0]
+
+
+# ---------------------------------------------------------------------------
+# standard and motif model estimation (tombo_stats.py:1236-1501, 1599-1740, 2108-2189)
+# ---------------------------------------------------------------------------
+# regions per tb2_kmer_level_summaries call (fewer when 64 regions exceed 2^24 positions)
+EST_REGION_BATCH = 64
+# command-line defaults of build_model estimate_reference / estimate_motif_alt_reference
+# (_option_parsers.py:290-291, 633-638, 911-913): --minimum-test-reads,
+# --coverage-threshold, --minimum-kmer-observations, --upstream-bases, --downstream-bases,
+# --multiprocess-region-size
+EST_REF_MIN_TEST_READS, EST_REF_COV_THRESH, EST_REF_MIN_KMER_OBS = 10, 100, 5
+EST_REF_UPSTRM_BASES, EST_REF_DNSTRM_BASES, EST_REF_REGION_SIZE = 1, 2, 10000
+
+
+def _open_read(r_data):
+    """the read's FAST5 file, opened read-only (the one place the estimation opens a read)"""
+    import h5py
+    return h5py.File(r_data.fn, 'r')
+
+
+def _read_slots(r_data):
+    """(genome-ordered norm_mean or None, read-centric bases or None) of one read"""
+    means, bases = th.get_multiple_slots_read_centric(r_data, ['norm_mean', 'base'],
+                                                      r_data.corr_group)
+    if means is not None:
+        means = np.asarray(means, dtype=np.float64)
+        if r_data.strand == '-':
+            means = means[::-1]
+    return means, bases
+
+
+def _update_seq(r_data, r_bases, reg_base_data, start, end):
+    """intervalData._update_seq tombo_helper.py:1891-1926, statement for statement"""
+    if r_bases is None:
+        th.warning_message(
+            'Unable to extract data from read. Potentially corrupted file ' +
+            'or invalid Tombo index file for this directory.')
+        return reg_base_data, max(0, r_data.start - start)
+    r_seq = b''.join(r_bases).decode()
+    if r_data.strand == '-':
+        r_seq = th.rev_comp(r_seq)
+    if r_data.start <= start:
+        r_end_overlap = r_data.end - start
+        if r_data.end > end:
+            r_end_clip = r_data.end - end
+            reg_base_data = r_seq[-r_end_overlap:-r_end_clip]
+            return reg_base_data, len(reg_base_data)
+        reg_base_data[:r_end_overlap] = r_seq[-r_end_overlap:]
+        return reg_base_data, r_end_overlap
+    if r_data.end > end:
+        r_begin_overlap = end - r_data.start
+        reg_base_data[-r_begin_overlap:] = r_seq[:r_begin_overlap]
+        return reg_base_data, len(reg_base_data)
+    r_len = r_data.end - r_data.start
+    r_int_start = r_data.start - start
+    reg_base_data[r_int_start:r_int_start + r_len] = r_seq
+    return reg_base_data, r_int_start + r_len
+
+
+def _interval_seq(reads, bases, start, end):
+    """intervalData.add_seq tombo_helper.py:1938-1974 from the reads (``bases`` maps each
+    read's position in ``reads`` to its bases); '-' where no read reaches"""
+    reg_base_data = ['-'] * (end - start)
+    if len(reads) == 0:
+        return ''.join(reg_base_data)
+    order = sorted(range(len(reads)), key=lambda i: (reads[i].start, reads[i].end))
+
+    def upd(i, data):
+        return _update_seq(reads[i], bases[i], data, start, end)
+    reg_base_data, curr_cov_pos = upd(order.pop(0), reg_base_data)
+    if len(order) == 0 or curr_cov_pos >= end - start:
+        return ''.join(reg_base_data)
+    curr = order.pop(0)
+    for nxt in order:
+        if reads[nxt].start >= curr_cov_pos:
+            reg_base_data, curr_cov_pos = upd(curr, reg_base_data)
+            curr = nxt
+            if curr_cov_pos >= end - start:
+                return ''.join(reg_base_data)
+            continue
+        if reads[nxt].end > reads[curr].end:
+            curr = nxt
+    reg_base_data, _ = upd(curr, reg_base_data)
+    return ''.join(reg_base_data)
+
+
+def _kmer_codes(seq, poss, kmer_width, rev):
+    """base-4 codes of seq[p:p + kmer_width] (reverse-complemented with ``rev``) for p in
+    ``poss``; -1 where the k-mer is short or holds a base other than ACGT"""
+    poss = np.asarray(poss, dtype=np.int64)
+    codes = _BASE_CODE[np.frombuffer(seq.encode(), dtype=np.uint8)].astype(np.int64)
+    pad = np.full(int(poss.max(initial=0)) + kmer_width, 255, dtype=np.int64)
+    pad[:codes.shape[0]] = codes[:pad.shape[0]]
+    key = np.zeros(poss.shape[0], dtype=np.int64)
+    bad = np.zeros(poss.shape[0], dtype=bool)
+    for j in range(kmer_width):
+        c = pad[poss + (kmer_width - 1 - j if rev else j)]
+        bad |= c > 3
+        key = key * 4 + ((3 - c) if rev else c)
+    key[bad] = -1
+    return key
+
+
+def _region_obs(reg, cov, cov_thresh, kmer_width, bb, region_size, motif, valid_poss):
+    """get_region_kmer_levels :1267-1348 for one region: (region positions, keys) of its
+    observations in the reference's order, or None where it returns None.  Keys are k-mer
+    codes, or code * kmer_width + offset with a motif or ``valid_poss``."""
+    chrm, strand, reg_start, reads, bases = reg
+    cov_intervals = np.where(np.diff(np.concatenate([[False], cov > cov_thresh])))[0]
+    if cov[-1] > cov_thresh:
+        cov_intervals = np.concatenate([cov_intervals, [region_size]])
+    if cov_intervals.shape[0] <= 1:
+        return None
+    ab = kmer_width - 1 - bb
+    all_pos, all_key = [], []
+    for cov_start, cov_end in cov_intervals.reshape(-1, 2):
+        int_seq = _interval_seq(reads, bases, reg_start + cov_start - bb, reg_start + cov_end + ab)
+        int_len = cov_end - cov_start
+        if valid_poss is None and motif is None:
+            poss, offsets = np.arange(int_len), None
+        else:
+            if valid_poss is not None:
+                if (chrm, strand) not in valid_poss:
+                    continue
+                mod = valid_poss[(chrm, strand)] - reg_start - cov_start
+                mod = mod[np.logical_and(np.greater_equal(mod, 0), np.less(mod, int_len))]
+            elif strand == '+':
+                mod = [m.start() + motif.mod_pos - 1 - bb for m in motif.motif_pat.finditer(int_seq)
+                       if 0 <= m.start() + motif.mod_pos - 1 - bb < int_len]
+            else:
+                mod = [m.start() + motif.motif_len - motif.mod_pos - bb
+                       for m in motif.rev_comp_pat.finditer(int_seq)
+                       if 0 <= m.start() + motif.motif_len - motif.mod_pos - bb < int_len]
+            int_poss = [(mod_pos - i_offset + bb, i_offset if strand == '+' else kmer_width - i_offset - 1)
+                        for mod_pos in mod for i_offset in range(kmer_width)
+                        if 0 <= mod_pos - i_offset + bb < int_len]
+            poss = np.array([p for p, _ in int_poss], dtype=np.int64)
+            offsets = np.array([o for _, o in int_poss], dtype=np.int64)
+        if poss.shape[0] == 0:
+            continue
+        key = _kmer_codes(int_seq, poss, kmer_width, strand == '-')
+        if offsets is not None:
+            # (kmer, offset) keys: without a motif the reference's dict has k-mer keys only,
+            # so every such look-up fails (KeyError) and the row is skipped
+            key = np.where(key >= 0, key * kmer_width + offsets, -1) if motif is not None else \
+                np.full(key.shape[0], -1, dtype=np.int64)
+        all_pos.append(poss + cov_start)
+        all_key.append(key)
+    if not all_pos:
+        return np.zeros(0, dtype=np.int64), np.zeros(0, dtype=np.int64)
+    return np.concatenate(all_pos), np.concatenate(all_key)
+
+
+def _est_keys(kmer_width, motif):
+    """the reference's reg_kmer_levels keys (:1283-1291) in its order, with their codes"""
+    kmers = [''.join(k) for k in itertools.product('ACGT', repeat=kmer_width)]
+    if motif is None:
+        return kmers, np.arange(len(kmers), dtype=np.int64)
+    keys = [(k, i_offset - 1) for k in kmers for i_offset in motif.find_mod_poss(k)]
+    return keys, np.array([_kmer_code(k) * kmer_width + o for k, o in keys], dtype=np.int64)
+
+
+def _sample_region_reads(reads, reg_start, reg_end, cs_cov_thresh, region_size):
+    """the cs_cov_thresh subsample of :1247-1260 (numpy's global RNG)"""
+    if cs_cov_thresh is None:
+        return reads
+    np.random.shuffle(reads)
+    cumm_num_bases = np.cumsum([max(r.end, reg_end) - min(r.start, reg_start) for r in reads])
+    hit = np.nonzero(cumm_num_bases >= region_size * cs_cov_thresh)[0]
+    return reads[:hit[0]] if hit.shape[0] else reads
+
+
+def extract_kmer_levels(reads_index, region_size, cov_thresh, upstrm_bases, dnstrm_bases,
+                        cs_cov_thresh, est_mean=False, num_processes=1, motif=None,
+                        valid_poss=None, device=0):
+    """tombo_stats.py:1398-1452 with get_region_kmer_levels :1242-1359 -> one dict per
+    region that gives levels, in ``iter_cov_regs`` order: ``{kmer: (n, 2) array}`` (or
+    ``{(kmer, offset): ...}`` with ``motif`` / ``valid_poss``) of per-position (level, sd)
+    rows, the reference's keys and row order.
+
+    Regions, subsamples, sequences and keys follow the reference on the host; the
+    per-position summaries of a batch of regions are one tb2_kmer_level_summaries call
+    (calc_med_sd, or c_mean_std with ``est_mean``, of the levels in read order).  The
+    cs_cov_thresh shuffles draw from numpy's global RNG and leave it as it was on entry, as
+    the reference's forked worker does.  A region where no read has levels, or where the
+    subsample keeps no read, is skipped (the reference's worker dies there and the regions
+    after it are lost).  ``num_processes`` is accepted; no process is started.  No region
+    with levels raises :class:`tombo_helper.TomboError` with the reference's message."""
+    kmer_width = upstrm_bases + dnstrm_bases + 1
+    keys, key_codes = _est_keys(kmer_width, motif)
+    key_index = np.full(4 ** kmer_width * (kmer_width if motif is not None else 1), -1, dtype=np.int64)
+    key_index[key_codes] = np.arange(key_codes.shape[0])
+    batch = max(1, min(EST_REGION_BATCH, (1 << 24) // region_size))
+    ctx = _lib.get_context(device)
+    rng_state = np.random.get_state()
+    all_reg_kmer_levels = []
+    try:
+        regs = []
+
+        def flush():
+            lv, off, st = [], [0], []
+            for j, (_, _, reg_start, reads, means, _) in enumerate(regs):
+                for r, m in zip(reads, means):
+                    a, b = max(reg_start, r.start), min(reg_start + region_size, r.end)
+                    if m is not None and b > a:
+                        lv.append(m[a - r.start:b - r.start])
+                        off.append(off[-1] + b - a)
+                        st.append(j * region_size + a - reg_start)
+            levels, sds, cov = ctx.kmer_level_summaries(
+                len(regs) * region_size,
+                (np.concatenate(lv) if lv else np.zeros(0), np.array(off), np.array(st, dtype=np.int64)),
+                cov_thresh, est_mean)
+            for j, (chrm, strand, reg_start, reads, _, bases) in enumerate(regs):
+                sl = slice(j * region_size, (j + 1) * region_size)
+                obs = _region_obs((chrm, strand, reg_start, reads, bases), cov[sl], cov_thresh,
+                                  kmer_width, upstrm_bases if strand == '+' else dnstrm_bases,
+                                  region_size, motif, valid_poss)
+                if obs is None:
+                    continue
+                pos, key = obs
+                idx = np.where(key >= 0, key_index[np.maximum(key, 0)], -1)
+                pos, idx = pos[idx >= 0], idx[idx >= 0]
+                order = np.argsort(idx, kind='stable')
+                pos, idx = pos[order] + j * region_size, idx[order]
+                vals = np.stack([levels[pos], sds[pos]], axis=1)
+                bounds = np.searchsorted(idx, np.arange(len(keys) + 1))
+                all_reg_kmer_levels.append(dict(
+                    (k, vals[bounds[i]:bounds[i + 1]]) for i, k in enumerate(keys)))
+            del regs[:]
+
+        for chrm, strand, reg_start in reads_index.iter_cov_regs(cov_thresh, region_size):
+            reg_end = reg_start + region_size
+            reads = [r for r in reads_index.get_cs_reads(chrm, strand)
+                     if not (r.start >= reg_end or r.end <= reg_start)]
+            if len(reads) == 0:
+                continue
+            reads = _sample_region_reads(reads, reg_start, reg_end, cs_cov_thresh, region_size)
+            slots = [_read_slots(r) for r in reads]
+            # get_reads_events tombo_helper.py:2227-2229: no levels from a read whose
+            # norm_mean does not span its mapping (its bases still give sequence)
+            means = [m if m is not None and m.shape[0] == r.end - r.start else None
+                     for r, (m, _) in zip(reads, slots)]
+            if all(m is None for m in means):
+                continue
+            regs.append((chrm, strand, reg_start, reads, means, [b for _, b in slots]))
+            if len(regs) == batch:
+                flush()
+        if regs:
+            flush()
+    finally:
+        np.random.set_state(rng_state)
+    if len(all_reg_kmer_levels) == 0:
+        raise th.TomboError(
+            'No genomic positions contain --minimum-test-reads. Consider ' +
+            'setting this option to a lower value.')
+    return all_reg_kmer_levels
+
+
+_NOT_COVERED = (
+    'is not covered at any poitions by --minimum-test-reads.\n\t\tConsider fitting to a '
+    'smaller k-mer via the --upstream-bases and --downstream-bases, or lowering '
+    '--minimum-test-reads.\n\t\tNote that this may result in a lower quality model.')
+
+
+def _tabulate(all_reg_kmer_levels, min_kmer_obs, keys, key_codes, n_codes, what, device):
+    """one tb2_kmer_medians call over every region's rows -> (counts, median levels,
+    median sds) per key, with the reference's two failures"""
+    codes, rows = [], []
+    for reg in all_reg_kmer_levels:
+        for k, c in zip(keys, key_codes):
+            v = np.asarray(reg[k], dtype=np.float64).reshape(-1, 2)
+            if v.shape[0]:
+                codes.append(np.full(v.shape[0], c, dtype=np.int64))
+                rows.append(v)
+    rows = np.concatenate(rows) if rows else np.zeros((0, 2))
+    cnt, med_lv, med_sd = _lib.get_context(device).kmer_medians(
+        n_codes, np.concatenate(codes) if codes else np.zeros(0, dtype=np.int64),
+        rows[:, 0], rows[:, 1])
+    cnt, med_lv, med_sd = cnt[key_codes], med_lv[key_codes], med_sd[key_codes]
+    for i in range(len(keys)):
+        if cnt[i] == 0:
+            raise th.TomboError('At least one ' + what + _NOT_COVERED)
+        if cnt[i] < min_kmer_obs:
+            raise th.TomboError(
+                'K-mers represeneted in fewer observations than requested in the provided '
+                'reads. Consider a shorter k-mer or providing more reads.\n\t' +
+                str(int(cnt.min())) + ' observations found in least common kmer.')
+    return med_lv, med_sd
+
+
+def tabulate_kmer_levels(all_reg_kmer_levels, min_kmer_obs, device=0):
+    """tombo_stats.py:1454-1501 -> ``[(kmer, median level, median sd)]`` in
+    ``itertools.product`` order; the medians of every k-mer are one tb2_kmer_medians call.
+    A k-mer without observations, or one with fewer than ``min_kmer_obs``, raises
+    :class:`tombo_helper.TomboError` with the reference's message (for the second, the
+    reference raises NameError; the message gives the fewest observations of any k-mer)."""
+    kmer_width = len(next(iter(all_reg_kmer_levels[0].keys())))
+    keys, key_codes = _est_keys(kmer_width, None)
+    med_lv, med_sd = _tabulate(all_reg_kmer_levels, min_kmer_obs, keys, key_codes,
+                               4 ** kmer_width, 'k-mer ', device)
+    return [(k, med_lv[i], med_sd[i]) for i, k in enumerate(keys)]
+
+
+def tabulate_mod_kmer_levels(all_reg_kmer_levels, min_kmer_obs, motif, device=0):
+    """tombo_stats.py:2108-2158 -> ``[(kmer, offset, median level, median sd)]`` over the
+    motif's (kmer, offset) keys in the reference's order, one tb2_kmer_medians call"""
+    kmer_width = len(next(iter(all_reg_kmer_levels[0].keys()))[0])
+    keys, key_codes = _est_keys(kmer_width, motif)
+    med_lv, med_sd = _tabulate(all_reg_kmer_levels, min_kmer_obs, keys, key_codes,
+                               4 ** kmer_width * kmer_width, 'modified k-mer ', device)
+    return [(k, o, med_lv[i], med_sd[i]) for i, (k, o) in enumerate(keys)]
+
+
+def _read_corr_factors(r_data, init_ref):
+    """get_read_corr_factors :1624-1667 of one read -> (shift, scale) correction factors"""
+    from . import resquiggle as rsqgl
+    upstrm_bases = init_ref.central_pos
+    dnstrm_bases = init_ref.kmer_width - init_ref.central_pos - 1
+    with _open_read(r_data) as fast5_data:
+        all_raw_signal = th.get_raw_read_slot(fast5_data)['Signal'][:]
+        event_starts, r_seq = th.get_multiple_slots_read_centric(
+            fast5_data, ('start', 'base'), r_data.corr_group)
+    if r_data.rna:
+        all_raw_signal = all_raw_signal[::-1]
+        if USE_RNA_EVENT_SCALE:
+            rsqgl_params = load_resquiggle_parameters(th.seqSampleType(RNA_SAMP_TYPE, True))
+            num_events = compute_num_events(all_raw_signal.shape[0], r_data.end - r_data.start,
+                                            rsqgl_params.mean_obs_per_event, MIN_EVENT_TO_SEQ_RATIO)
+            valid_cpts = th.valid_cpts_w_cap_t_test(
+                all_raw_signal.astype(np.float64), rsqgl_params.min_obs_per_base,
+                rsqgl_params.running_stat_width, num_events)
+            if COLLAPSE_RNA_STALLS:
+                valid_cpts = rsqgl._remove_stall_cpts(identify_stalls(all_raw_signal), valid_cpts)
+            scale_values = rsqgl._rna_event_scale_values(all_raw_signal, valid_cpts, OUTLIER_THRESH)
+            norm_signal, scale_values = normalize_raw_signal(all_raw_signal, scale_values=scale_values)
+        else:
+            norm_signal, scale_values = normalize_raw_signal(all_raw_signal)
+    else:
+        norm_signal, scale_values = normalize_raw_signal(all_raw_signal)
+    event_starts = np.asarray(event_starts).astype(np.int64)
+    rsrtr = r_data.read_start_rel_to_raw + event_starts[upstrm_bases]
+    if dnstrm_bases > 1:
+        event_starts = event_starts[upstrm_bases:-(dnstrm_bases - 1)]
+    else:
+        assert dnstrm_bases == 1, (
+            'Must have at least one upstream and downstream base for a Tombo model.')
+        event_starts = event_starts[upstrm_bases:]
+    event_starts -= event_starts[0]
+    norm_signal = norm_signal[rsrtr:rsrtr + event_starts[-1]]
+    r_seq = b''.join(r_seq).decode()
+    r_ref_means, _ = init_ref.get_exp_levels_from_seq(r_seq)
+    _, _, shift_corr_factor, scale_corr_factor = calc_kmer_fitted_shift_scale(
+        scale_values.shift, scale_values.scale, compute_base_means(norm_signal, event_starts),
+        r_ref_means, method='theil_sen')
+    return shift_corr_factor, scale_corr_factor
+
+
+def center_model_to_median_norm(reads_index, init_ref, max_reads=NUM_READS_TO_ADJUST_MODEL):
+    """tombo_stats.py:1599-1705: shuffle the reads (numpy's global RNG), fit each read's
+    Theil-Sen shift and scale correction against ``init_ref`` (normalisation, base means and
+    the fit through the device entry points) until ``max_reads`` reads succeed, then center
+    ``init_ref`` in place on the medians of the factors and return it.  A read that raises
+    is skipped; fewer than ``max_reads`` reads warns, none raises
+    :class:`tombo_helper.TomboError` with the reference's messages."""
+    all_shift_corr_factors, all_scale_corr_factors = [], []
+    all_reads = list(reads_index.iter_reads())
+    np.random.shuffle(all_reads)
+    for r_data in all_reads:
+        try:
+            r_shift, r_scale = _read_corr_factors(r_data, init_ref)
+        except Exception:
+            continue
+        all_shift_corr_factors.append(r_shift)
+        all_scale_corr_factors.append(r_scale)
+        if len(all_shift_corr_factors) >= max_reads:
+            break
+    if len(all_shift_corr_factors) < max_reads:
+        if len(all_shift_corr_factors) == 0:
+            raise th.TomboError(
+                'No reads succcessfully processed for sequence-based ' +
+                'normalization parameter re-fitting.')
+        th.warning_message(
+            'Fewer reads succcessfully processed for sequence-based ' +
+            'normalization parameter re-fitting than requested.')
+    init_ref._center_model(np.median(all_shift_corr_factors), np.median(all_scale_corr_factors))
+    return init_ref
+
+
+def _check_context(upstrm_bases, dnstrm_bases):
+    if min(upstrm_bases, dnstrm_bases) == 0:
+        raise th.TomboError('Context upstream and downstream must be greater ' +
+                            'than 0 for model estimation.')
+
+
+def estimate_kmer_model(reads_index, cov_thresh, upstrm_bases, dnstrm_bases, min_kmer_obs,
+                        kmer_specific_sd, cs_cov_thresh, est_mean, region_size, num_processes=1):
+    """tombo_stats.py:1716-1740 (with _est_ref_main's context check :4788-4791) on a reads
+    index -> the centered standard :class:`TomboModel`"""
+    _check_context(upstrm_bases, dnstrm_bases)
+    all_reg_kmer_levels = extract_kmer_levels(
+        reads_index, region_size, cov_thresh, upstrm_bases, dnstrm_bases, cs_cov_thresh,
+        est_mean, num_processes)
+    all_kmer_mean_sds = tabulate_kmer_levels(all_reg_kmer_levels, min_kmer_obs)
+    init_ref = TomboModel(kmer_ref=all_kmer_mean_sds, central_pos=upstrm_bases)
+    centered_ref = center_model_to_median_norm(reads_index, init_ref)
+    if not kmer_specific_sd:
+        centered_ref._make_constant_sd()
+    return centered_ref
+
+
+def estimate_motif_alt_model(reads_index, motif_desc, upstrm_bases, dnstrm_bases, valid_poss,
+                             min_kmer_obs, cov_thresh, cs_cov_thresh, region_size,
+                             num_processes=1):
+    """tombo_stats.py:2160-2189 on a reads index, with ``valid_poss`` as
+    :func:`tombo_helper.parse_locs_file` returns it (or None) -> :class:`AltModel`"""
+    _check_context(upstrm_bases, dnstrm_bases)
+    try:
+        raw_motif, mod_pos = motif_desc.split(':')
+        mod_pos = int(mod_pos)
+    except Exception:
+        raise th.TomboError('Invalid motif decription format.')
+    motif = th.TomboMotif(raw_motif, mod_pos)
+    all_reg_kmer_levels = extract_kmer_levels(
+        reads_index, region_size, cov_thresh, upstrm_bases, dnstrm_bases, cs_cov_thresh,
+        False, num_processes, motif, valid_poss)
+    all_mod_kmer_mean_sds = tabulate_mod_kmer_levels(all_reg_kmer_levels, min_kmer_obs, motif)
+    alt_ref = AltModel(kmer_ref=all_mod_kmer_mean_sds, central_pos=upstrm_bases,
+                       alt_base=motif.mod_base, motif=motif)
+    alt_ref._make_constant_sd()
+    return alt_ref
