@@ -17,7 +17,7 @@
  *     _c_dynamic_programming.pyx:9-13, _c_helper.pyx:6-13).
  *   - every call returns 0 (TB2_OK) or a TB2_ERR_* code; per-read outcomes of
  *     batched calls are reported in a status array with the same codes.  Codes
- *     1..22 map 1:1 onto the reference's TomboError / NotImplementedError message
+ *     1..25 map 1:1 onto the reference's TomboError / NotImplementedError message
  *     strings (tb2_status_message); the reference raises, we return.
  *   - there is NO CPU fallback: every entry point runs CUDA kernels and fails with
  *     TB2_ERR_CUDA if no sm_90-class device is usable.
@@ -56,6 +56,9 @@ enum {
     TB2_ERR_THEIL_SEN_ZERO = 20,        /* tombo_stats.py:421 */
     TB2_ERR_INVALID_START_PATH = 21,    /* tombo_stats.py:2356 */
     TB2_ERR_READ_TOO_SHORT_IN_REGION = 22,  /* tombo_stats.py:3944 */
+    TB2_ERR_NO_INFO_IN_REGION = 23,     /* tombo_stats.py:3839-3841 */
+    TB2_ERR_FISHER_TOO_SHORT = 24,      /* tombo_stats.py:2257-2259 */
+    TB2_ERR_NO_VALID_Z = 25,            /* tombo_stats.py:3757-3758 */
     TB2_ERR_UNEXPECTED = 100,  /* the reference would raise a non-Tombo exception */
     /* library level */
     TB2_ERR_CUDA = 200,        /* CUDA runtime failure (see tb2_last_error) */
@@ -119,7 +122,8 @@ int64_t tb2_launch_count(tb2_ctx *ctx);
  * out[0] whole compute stage, out[1] sum over launches of the dominant kernel
  * (banded DP, k_align), out[2] number of k_align launches, out[3] reads
  * processed summed over those launches.  After tb2_group_reg_stats / tb2_reads_ref_levels /
- * tb2_kmer_level_summaries / tb2_kmer_medians:
+ * tb2_kmer_level_summaries / tb2_kmer_medians / tb2_de_novo_read_stats_batch /
+ * tb2_de_novo_region_stats / tb2_sample_compare_region_stats / tb2_batch_de_novo_region:
  * out[0] is the device time from the call's first kernel to its last (upload and download
  * excluded), out[1..3] are 0.  After tb2_kernel_densities: out[0] likewise, out[1] the part
  * of it spent in the per-set setup kernel (std, factor, kernel width), out[2..3] 0 */
@@ -436,6 +440,63 @@ int tb2_de_novo_read_stats_batch(tb2_ctx *ctx, int64_t n_reads, const double *no
                                  const int64_t *seq_off, const int64_t *read_start,
                                  int64_t fm_offset, double *pvals_out, int64_t *pos_out,
                                  int64_t *stat_off);
+
+/* ---- de novo / sample-compare tests of one region, both strands ----------------------
+ * compute_reg_stats (tombo_stats.py:4180-4229) runs one per-read test per read of a region
+ * block; these run it for n_reads reads over [reg_start, reg_end) in one call.  strand[r]:
+ * 0 '+', 1 '-', -1 skip the read (no statistics, status 0).  Read data are read-centric as
+ * the reference stores them; read_start[r] is the genome's low coordinate on both strands and
+ * the read ends at read_start[r] + nb.  Outputs are laid out by stat_off (n_reads + 1,
+ * filled); pvals_out / pos_out hold up to sum(nb) entries.  read_status (nullable, n_reads)
+ * gets 0 or the code of the TomboError the reference raises for the read; such a read has no
+ * statistics.  The statistics also stay on the device for tb2_region_stats_add_tests, until
+ * the next call of either function or of tb2_batch_de_novo_region.  fm_offset 0 .. 64.
+ * tb2_last_timing out[0] is the kernel time.
+ *
+ * tb2_de_novo_region_stats: compute_de_novo_read_stats (:3771-3873) with the canonical model
+ * (tb2_set_model) in the layout of tb2_alt_model_llr_motif_batch (nb + K - 1 codes per read,
+ * the read's bases from code cpos).  Per read: the clip by the strand's k-mer lags plus
+ * fm_offset, with Python's slicing (a clip longer than the read empties it); k-mers of the
+ * clipped bases, reversed for '-' reads; means flipped to genome order and trimmed by the
+ * lags; z -> two-sided p -> Fisher window -> max(p, SMALLEST_PVAL).  Positions ascend on
+ * both strands; the window's NaN edges are kept.  r_means[begin:-0] is empty when the end
+ * lag is 0 (central_pos == K - 1 on '+', 0 on '-'): such a read has no statistics.
+ * Statuses: TB2_ERR_NO_INFO_IN_REGION (fewer than K clipped bases), TB2_ERR_INVALID_SEQ
+ * (a non-ACGT code or a k-mer absent from the model among the clipped bases' k-mers; codes
+ * outside them are never read), TB2_ERR_FISHER_TOO_SHORT.
+ *
+ * tb2_sample_compare_region_stats: compute_sample_compare_read_stats (:3675-3769) against
+ * ctrl_means / ctrl_sds over [reg_start - fm_offset, reg_end + fm_offset) (get_reads_ref).
+ * Per read: the clip by fm_offset, flip, z against the control slice, p (no clamp), the
+ * Fisher window; only the non-NaN entries are returned, in genome order.  Statuses:
+ * TB2_ERR_NO_VALID_Z, TB2_ERR_FISHER_TOO_SHORT.
+ *
+ * TB2_ERR_INVALID_ARG: a strand outside {-1, 0, 1}, fm_offset outside 0 .. 64,
+ * reg_end <= reg_start, NULL ctrl_* (sample compare), a code count that is not nb + K - 1 or
+ * no model set (de novo). */
+int tb2_de_novo_region_stats(tb2_ctx *ctx, int64_t n_reads, const double *norm_mean,
+                             const int64_t *mean_off, const uint8_t *seq, const int64_t *seq_off,
+                             const int64_t *read_start, const int8_t *strand, int64_t fm_offset,
+                             int64_t reg_start, int64_t reg_end, double *pvals_out,
+                             int64_t *pos_out, int64_t *stat_off, int32_t *read_status);
+int tb2_sample_compare_region_stats(tb2_ctx *ctx, int64_t n_reads, const double *norm_mean,
+                                    const int64_t *mean_off, const int64_t *read_start,
+                                    const int8_t *strand, const double *ctrl_means,
+                                    const double *ctrl_sds, int64_t fm_offset, int64_t reg_start,
+                                    int64_t reg_end, double *pvals_out, int64_t *pos_out,
+                                    int64_t *stat_off, int32_t *read_status);
+/* the de novo test on the RESIDENT batch (after tb2_batch_compute): read_start / strand have
+ * one entry per read of the batch.  Reads whose resquiggle failed report that status (also at
+ * strand -1) and feed nothing to the counters; their outputs are NaN.  pvals_out / pos_out /
+ * stat_off / read_status may be NULL: the statistics stay on the device for
+ * tb2_region_stats_add_tests, so resquiggle -> de novo -> region counts never leaves HBM. */
+int tb2_batch_de_novo_region(tb2_ctx *ctx, const int64_t *read_start, const int8_t *strand,
+                             int64_t fm_offset, int64_t reg_start, int64_t reg_end,
+                             double *pvals_out, int64_t *pos_out, int64_t *stat_off,
+                             int32_t *read_status);
+/* accumulate the statistics of the last de novo / sample-compare region call into the open
+ * region (tb2_region_stats_begin) as stat_type 1; lower_thresh NaN <=> None */
+int tb2_region_stats_add_tests(tb2_ctx *ctx, double single_read_thresh, double lower_thresh);
 
 /* ---- level_sample_compare and control-sample reference levels ------------------------
  * One region [reg_start, reg_start + reg_len) per call, already widened by fm_offset

@@ -136,6 +136,12 @@ _PROTOS = {
     'tb2_window_fisher_pvals': (_I, [_CTX, i64, pF64, pF64, pF64, pI64, i64, _I, pF64]),
     'tb2_de_novo_read_stats_batch': (_I, [_CTX, i64, pF64, pI64, pU8, pI64, pI64, i64, pF64, pI64,
                                           pI64]),
+    'tb2_de_novo_region_stats': (_I, [_CTX, i64, pF64, pI64, pU8, pI64, pI64, pI8, i64, i64, i64,
+                                      pF64, pI64, pI64, pI32]),
+    'tb2_sample_compare_region_stats': (_I, [_CTX, i64, pF64, pI64, pI64, pI8, pF64, pF64, i64, i64,
+                                             i64, pF64, pI64, pI64, pI32]),
+    'tb2_batch_de_novo_region': (_I, [_CTX, pI64, pI8, i64, i64, i64, pF64, pI64, pI64, pI32]),
+    'tb2_region_stats_add_tests': (_I, [_CTX, f64, f64]),
     'tb2_group_reg_stats': (_I, [_CTX, i64, i64, i64, pF64, pI64, pI64, i64, pF64, pI64, pI64, _I,
                                  _I, i64, i64, i64, pI64, pF64, pI64, pI64, pI64]),
     'tb2_reads_ref_levels': (_I, [_CTX, i64, i64, i64, pF64, pI64, pI64, i64, _I, pF64, pF64, f64,
@@ -759,6 +765,79 @@ class Context(object):
             ptr(stat_off, i64)))
         t = int(stat_off[-1])
         return pv[:t].copy(), pos[:t].copy(), stat_off
+
+    def de_novo_region_stats(self, norm_mean, mean_off, seq, seq_off, read_start, strand,
+                             fm_offset, reg_start, reg_end):
+        """tb2_de_novo_region_stats -> (pvals, pos, stat_off, read_status); the statistics
+        also stay on the device for region_stats_add_tests"""
+        norm_mean, mean_off = as_f64(norm_mean), as_i64(mean_off)
+        seq = np.ascontiguousarray(seq, dtype=np.uint8)
+        seq_off, read_start = as_i64(seq_off), as_i64(read_start)
+        strand = np.ascontiguousarray(strand, dtype=np.int8)
+        n = mean_off.shape[0] - 1
+        cap = max(1, norm_mean.shape[0])
+        pv, pos = np.empty(cap), np.empty(cap, dtype=np.int64)
+        stat_off = np.zeros(n + 1, dtype=np.int64)
+        status = np.zeros(max(1, n), dtype=np.int32)
+        self.check(self.lib.tb2_de_novo_region_stats(
+            self.handle, n, ptr(norm_mean, f64), ptr(mean_off, i64), ptr(seq, C.c_uint8),
+            ptr(seq_off, i64), ptr(read_start, i64), ptr(strand, C.c_int8), int(fm_offset),
+            int(reg_start), int(reg_end), ptr(pv, f64), ptr(pos, i64), ptr(stat_off, i64),
+            ptr(status, C.c_int32)))
+        t = int(stat_off[-1])
+        return pv[:t].copy(), pos[:t].copy(), stat_off, status[:n].copy()
+
+    def sample_compare_region_stats(self, norm_mean, mean_off, read_start, strand, ctrl_means,
+                                    ctrl_sds, fm_offset, reg_start, reg_end):
+        """tb2_sample_compare_region_stats -> (pvals, pos, stat_off, read_status); ctrl_*
+        cover [reg_start - fm_offset, reg_end + fm_offset)"""
+        norm_mean, mean_off, read_start = as_f64(norm_mean), as_i64(mean_off), as_i64(read_start)
+        strand = np.ascontiguousarray(strand, dtype=np.int8)
+        ctrl_means, ctrl_sds = as_f64(ctrl_means), as_f64(ctrl_sds)
+        if not ctrl_means.shape[0] == ctrl_sds.shape[0] == int(reg_end) - int(reg_start) + 2 * int(fm_offset):
+            raise ValueError('control levels must cover [reg_start - fm_offset, reg_end + fm_offset)')
+        n = mean_off.shape[0] - 1
+        cap = max(1, norm_mean.shape[0])
+        pv, pos = np.empty(cap), np.empty(cap, dtype=np.int64)
+        stat_off = np.zeros(n + 1, dtype=np.int64)
+        status = np.zeros(max(1, n), dtype=np.int32)
+        self.check(self.lib.tb2_sample_compare_region_stats(
+            self.handle, n, ptr(norm_mean, f64), ptr(mean_off, i64), ptr(read_start, i64),
+            ptr(strand, C.c_int8), ptr(ctrl_means, f64), ptr(ctrl_sds, f64), int(fm_offset),
+            int(reg_start), int(reg_end), ptr(pv, f64), ptr(pos, i64), ptr(stat_off, i64),
+            ptr(status, C.c_int32)))
+        t = int(stat_off[-1])
+        return pv[:t].copy(), pos[:t].copy(), stat_off, status[:n].copy()
+
+    def batch_de_novo_region(self, read_start, strand, fm_offset, reg_start, reg_end,
+                             download=True):
+        """de novo test of the resident batch (after batch_compute) -> (pvals, pos, stat_off,
+        read_status); with download=False the statistics stay on the device only and
+        (None, None, stat_off, read_status) is returned"""
+        read_start = as_i64(read_start)
+        strand = np.ascontiguousarray(strand, dtype=np.int8)
+        n = self._base_off.shape[0] - 1 if getattr(self, '_base_off', None) is not None else -1
+        if read_start.shape != (n,) or strand.shape != (n,):
+            raise ValueError('read_start and strand need one entry per read of the resident '
+                             'batch (%d)' % n)
+        cap = max(1, int(self._base_off[-1]))
+        pv = np.empty(cap) if download else None
+        pos = np.empty(cap, dtype=np.int64) if download else None
+        stat_off = np.zeros(n + 1, dtype=np.int64)
+        status = np.zeros(max(1, n), dtype=np.int32)
+        self.check(self.lib.tb2_batch_de_novo_region(
+            self.handle, ptr(read_start, i64), ptr(strand, C.c_int8), int(fm_offset),
+            int(reg_start), int(reg_end), ptr(pv, f64) if download else None,
+            ptr(pos, i64) if download else None, ptr(stat_off, i64), ptr(status, C.c_int32)))
+        t = int(stat_off[-1])
+        if not download:
+            return None, None, stat_off, status[:n].copy()
+        return pv[:t].copy(), pos[:t].copy(), stat_off, status[:n].copy()
+
+    def region_stats_add_tests(self, single_read_thresh, lower_thresh=None):
+        """accumulate the last de novo / sample-compare region call into the open region"""
+        self.check(self.lib.tb2_region_stats_add_tests(
+            self.handle, single_read_thresh, float('nan') if lower_thresh is None else lower_thresh))
 
     def kernel_densities(self, levels, off, x, bw):
         """tb2_kernel_densities -> (densities (n_sets, len(x)), cho_cov, factor).  Set s is

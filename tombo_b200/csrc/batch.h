@@ -106,6 +106,7 @@ struct BatchResultView {
     const unsigned char *seq;
     const int *status;                  // status[r * stride]
     int stride;
+    const long long *host_base_off;     // host copy of base_off (n_reads + 1)
 };
 int tb2_batch_result_view(tb2_ctx *ctx, BatchResultView *out);
 int tb2_region_accumulate_dev(tb2_ctx *ctx, long long n, const double *stats_dev,

@@ -568,6 +568,7 @@ int tb2_batch_result_view(tb2_ctx *ctx, BatchResultView *out)
     out->seq = h->v.seq;
     out->status = &h->v.st[0].status;
     out->stride = (int)(sizeof(ReadState) / sizeof(int));
+    out->host_base_off = h->hb.base_off.data();
     return TB2_OK;
 }
 

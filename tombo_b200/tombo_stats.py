@@ -13,6 +13,7 @@ import re
 import numpy as np
 
 from . import _lib
+from . import formats
 from . import tombo_helper as th
 from ._default_parameters import (
     ALGN_PARAMS_TABLE, SEG_PARAMS_TABLE, RNA_SAMP_TYPE, DNA_SAMP_TYPE,
@@ -33,7 +34,8 @@ __all__ = [
     'parse_base_levels', 'est_kernel_density', 'write_kmer_densities_file',
     'parse_kmer_densities_file', 'isolate_alt_density', 'extract_kmer_levels',
     'tabulate_kmer_levels', 'tabulate_mod_kmer_levels', 'center_model_to_median_norm',
-    'estimate_kmer_model', 'estimate_motif_alt_model']
+    'estimate_kmer_model', 'estimate_motif_alt_model', 'compute_de_novo_reads_stats',
+    'compute_sample_compare_reads_stats', 'compute_reg_stats']
 
 # E|N(0,1)| = sqrt(2 / pi); the reference evaluates scipy.stats.halfnorm.expect()
 # (tombo_stats.py:84), which returns this value (SURVEY.md 8c-2)
@@ -688,6 +690,180 @@ def compute_sample_compare_read_stats(r_data, ctrl_means, ctrl_sds, fm_offset=FM
         np.ascontiguousarray(r_means), cm, cs, np.array([0, r_means.shape[0]]), fm_offset, False)
     r_poss = np.where(~np.isnan(r_pvals))[0]
     return {SAMP_COMP_TXT: r_pvals[r_poss]}, {SAMP_COMP_TXT: r_poss + read_start}, read_id
+
+
+def _read_id(r_data):
+    try:
+        return th.get_raw_read_slot(r_data).attrs.get('read_id')
+    except Exception:
+        return getattr(r_data, 'read_id', None)
+
+
+def _region_bounds(reg_data, starts, nbs):
+    if reg_data is not None:
+        return reg_data.start, reg_data.end
+    # a region that contains every read leaves each one whole
+    return int(starts.min()), int((starts + nbs).max())
+
+
+def _per_read_results(out, idx, ids, stat_name, pv, pos, stat_off, status):
+    for j, i in enumerate(idx):
+        if status[j] != 0:
+            out[i] = th.TomboError(_lib.status_message(status[j]))
+        else:
+            a, b = int(stat_off[j]), int(stat_off[j + 1])
+            out[i] = ({stat_name: pv[a:b]}, {stat_name: pos[a:b]}, ids[j])
+    return out
+
+
+def compute_de_novo_reads_stats(r_datas, std_ref, fm_offset, reg_data, device=0):
+    """Batched :func:`compute_de_novo_read_stats`: every read of ``r_datas`` (either strand),
+    clipped to ``reg_data`` (None: whole reads), in one device call.  Read data arrive through
+    the same FAST5 seam.  Returns, per read, ``({'de_novo': p-values}, {'de_novo': positions},
+    read_id)`` or the :class:`tombo_helper.TomboError` the reference would raise for it.  The
+    statistics stay on the device for ``Context.region_stats_add_tests``.
+
+    A non-ACGT base or a k-mer absent from the model among the k-mers the clipped read uses
+    gives 'Invalid sequence encountered from genome sequence.' (the reference exits).  Where
+    ``r_means[begin:-0]`` empties the levels (central_pos == K - 1 on '+', 0 on '-') the read
+    has neither p-values nor positions.  A read whose base and level counts differ fails with
+    'Mismatching k-mer and mean levels.'.  ``fm_offset`` above 64 raises
+    ``_lib.TomboB200Error``."""
+    K, cpos = std_ref.kmer_width, std_ref.central_pos
+    out = [None] * len(r_datas)
+    means, codes, starts, strands, ids, idx = [], [], [], [], [], []
+    for i, r_data in enumerate(r_datas):
+        r_means, r_seq = th.get_multiple_slots_read_centric(
+            r_data, ['norm_mean', 'base'], r_data.corr_group)
+        read_id = _read_id(r_data)
+        if r_means is None or r_seq is None:
+            out[i] = th.TomboError('Read does not contain valid re-squiggled data.')
+            continue
+        r_seq = b''.join(r_seq) if not isinstance(r_seq, str) else r_seq.encode()
+        c = _BASE_CODE[np.frombuffer(r_seq, dtype=np.uint8)]
+        r_means = np.asarray(r_means, dtype=np.float64)
+        if c.shape[0] != r_means.shape[0]:
+            out[i] = th.TomboError('Mismatching k-mer and mean levels.')
+            continue
+        # the library's layout: nb + K - 1 codes, the read's bases cpos codes in; codes
+        # outside the clipped bases are never read
+        means.append(r_means)
+        codes.append(np.concatenate([np.zeros(cpos, np.uint8), c, np.zeros(K - 1 - cpos, np.uint8)]))
+        starts.append(r_data.start)
+        strands.append(0 if r_data.strand == '+' else 1)
+        ids.append(read_id)
+        idx.append(i)
+    if not idx:
+        return out
+    nbs = np.array([m.shape[0] for m in means], dtype=np.int64)
+    starts = np.array(starts, dtype=np.int64)
+    reg_start, reg_end = _region_bounds(reg_data, starts, nbs)
+    ctx = _lib.get_context(device)
+    _lib.ensure_model(ctx, std_ref)
+    pv, pos, stat_off, status = ctx.de_novo_region_stats(
+        np.concatenate(means), np.concatenate([[0], np.cumsum(nbs)]), np.concatenate(codes),
+        np.concatenate([[0], np.cumsum(nbs + K - 1)]), starts, np.array(strands, dtype=np.int8),
+        fm_offset, reg_start, reg_end)
+    return _per_read_results(out, idx, ids, DE_NOVO_TXT, pv, pos, stat_off, status)
+
+
+def compute_sample_compare_reads_stats(r_datas, ctrl_means, ctrl_sds, fm_offset, reg_data,
+                                       device=0):
+    """Batched :func:`compute_sample_compare_read_stats` over ``r_datas`` (either strand) in
+    one device call; ``ctrl_means`` / ``ctrl_sds`` cover [reg_start - fm_offset,
+    reg_end + fm_offset) as ``get_reads_ref`` returns them.  Returns, per read,
+    ``({'sample_compare': p-values}, {...: positions}, read_id)`` (the non-NaN entries) or the
+    :class:`tombo_helper.TomboError` the reference would raise.  The statistics stay on the
+    device for ``Context.region_stats_add_tests``."""
+    out = [None] * len(r_datas)
+    means, starts, strands, ids, idx = [], [], [], [], []
+    for i, r_data in enumerate(r_datas):
+        got = th.get_multiple_slots_read_centric(r_data, ['norm_mean'], r_data.corr_group)
+        r_means = got[0] if isinstance(got, (tuple, list)) else got
+        read_id = _read_id(r_data)
+        if r_means is None:
+            out[i] = th.TomboError('Read does not contain re-squiggled level means.')
+            continue
+        means.append(np.asarray(r_means, dtype=np.float64))
+        starts.append(r_data.start)
+        strands.append(0 if r_data.strand == '+' else 1)
+        ids.append(read_id)
+        idx.append(i)
+    if not idx:
+        return out
+    nbs = np.array([m.shape[0] for m in means], dtype=np.int64)
+    starts = np.array(starts, dtype=np.int64)
+    if reg_data is None:
+        raise NotImplementedError('control levels are given for one region: reg_data is needed')
+    ctx = _lib.get_context(device)
+    pv, pos, stat_off, status = ctx.sample_compare_region_stats(
+        np.concatenate(means), np.concatenate([[0], np.cumsum(nbs)]), starts,
+        np.array(strands, dtype=np.int8), ctrl_means, ctrl_sds, fm_offset, reg_data.start,
+        reg_data.end)
+    return _per_read_results(out, idx, ids, SAMP_COMP_TXT, pv, pos, stat_off, status)
+
+
+def compute_reg_stats(reg_data, fm_offset, min_test_reads, single_read_thresh, lower_thresh,
+                      ctrl_reg_data, std_ref, alt_refs, use_standard_llhr, per_read_q, stat_type,
+                      prior_weights):
+    """tombo_stats.py:4180-4229 -> ``[(stat_name, tombo_helper.regionStats)]``.  De novo and
+    sample-compare make one region call for all reads of the block and feed the region
+    counters from the statistics left on the device; model_compare makes one call per
+    alternative model.  Reads that fail with a TomboError are skipped.  With ``per_read_q``
+    the per-read block of each statistic is queued as the reference queues it (:4152-4154);
+    its read-id lookup is in first-seen order (the reference's follows ``set`` iteration)."""
+    ctx = _lib.get_context()
+    ctrl_cov = None
+    if stat_type == SAMP_COMP_TXT:
+        ctrl_means, ctrl_sds, ctrl_cov = get_reads_ref(
+            ctrl_reg_data, min_test_reads, fm_offset, std_ref, prior_weights)
+        results = compute_sample_compare_reads_stats(
+            reg_data.reads, ctrl_means, ctrl_sds, fm_offset, reg_data)
+    elif stat_type == DE_NOVO_TXT:
+        results = compute_de_novo_reads_stats(reg_data.reads, std_ref, fm_offset, reg_data)
+    else:
+        results = compute_alt_model_reads_stats(
+            reg_data.reads, std_ref, alt_refs, use_standard_llhr, reg_data)
+    stat_names = [stat_type] if stat_type != ALT_MODEL_TXT else list(zip(*alt_refs))[0]
+    reg_read_stats, stat_locs, reg_ids = [dict((n, []) for n in stat_names) for _ in range(3)]
+    for res in results:
+        if isinstance(res, th.TomboError) or res[0] is None:
+            continue
+        r_stats, r_poss, read_id = res
+        for stat_name, stat_r_stats in r_stats.items():
+            reg_read_stats[stat_name].append(stat_r_stats)
+            reg_ids[stat_name].append((read_id, stat_r_stats.shape[0]))
+            stat_locs[stat_name].append(r_poss[stat_name])
+    if sum(len(v) for v in reg_read_stats.values()) == 0:
+        raise th.TomboError('Reads contains no statistics in this region.')
+    reg_stats = []
+    for stat_name, stats in reg_read_stats.items():
+        if per_read_q is not None:
+            block, lookup = formats.per_read_block(stats, stat_locs[stat_name], reg_ids[stat_name])
+            per_read_q.put((stat_name, (block, lookup, reg_data.chrm, reg_data.strand,
+                                        reg_data.start)))
+        if stat_type == ALT_MODEL_TXT:
+            reg_stats.append((stat_name, collate_reg_stats(
+                stats, stat_locs[stat_name], reg_ids[stat_name], None, reg_data,
+                single_read_thresh, lower_thresh, stat_type, stat_name, ctrl_cov)))
+            continue
+        # the statistics of the region call are still on the device
+        ctx.region_stats_begin(reg_data.start, reg_data.end - reg_data.start)
+        ctx.region_stats_add_tests(single_read_thresh, lower_thresh)
+        agg = ctx.region_stats_finalize()
+        if agg['pos'].shape[0] == 0:
+            raise th.TomboError('No valid positions in this region.')
+        # one ctrl_cov entry per sorted statistic, as apply_per_read_thresh builds it
+        sorted_locs = np.repeat(agg['pos'], agg['cov'])
+        if stat_type == SAMP_COMP_TXT:
+            cc = [ctrl_cov[pos] if ctrl_cov is not None and pos in ctrl_cov else 0
+                  for pos in sorted_locs]
+        else:
+            cc = [0] * int(sorted_locs.shape[0])
+        reg_stats.append((stat_name, th.regionStats(
+            agg['frac'], agg['pos'], reg_data.chrm, reg_data.strand, reg_data.start, agg['cov'],
+            cc, agg['valid_cov'])))
+    return reg_stats
 
 
 # ---------------------------------------------------------------------------
