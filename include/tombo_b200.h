@@ -123,7 +123,8 @@ int64_t tb2_launch_count(tb2_ctx *ctx);
  * (banded DP, k_align), out[2] number of k_align launches, out[3] reads
  * processed summed over those launches.  After tb2_group_reg_stats / tb2_reads_ref_levels /
  * tb2_kmer_level_summaries / tb2_kmer_medians / tb2_de_novo_read_stats_batch /
- * tb2_de_novo_region_stats / tb2_sample_compare_region_stats / tb2_batch_de_novo_region:
+ * tb2_de_novo_region_stats / tb2_sample_compare_region_stats / tb2_batch_de_novo_region /
+ * tb2_accuracy_label_motif / _truth / _ctrl / tb2_accuracy_curve / tb2_accuracy_rates_ordered:
  * out[0] is the device time from the call's first kernel to its last (upload and download
  * excluded), out[1..3] are 0.  After tb2_kernel_densities: out[0] likewise, out[1] the part
  * of it spent in the per-set setup kernel (std, factor, kernel width), out[2..3] 0 */
@@ -582,6 +583,71 @@ int tb2_kmer_level_summaries(tb2_ctx *ctx, int64_t n_pos, int64_t n_reads, const
 int tb2_kmer_medians(tb2_ctx *ctx, int64_t n_keys, int64_t n_obs, const int64_t *keys,
                      const double *levels, const double *sds, int64_t *count_out,
                      double *level_med_out, double *sd_med_out);
+
+/* ---- accuracy of modified-base calls (tombo plot roc and friends) ------ */
+/* Labelling appends (stat, label) entries to slots 0 .. 15 (one per modification name) that
+ * stay on the device until tb2_accuracy_reset; tb2_accuracy_curve turns a slot into the
+ * sampled rates of prep_accuracy_rates (_plot_commands.py:60-82).
+ *
+ * One statistics block (chrm, strand, start, end, block_stats) of the stats iterator:
+ * its reg_seq as codes seq[seq_off .. seq_off + seq_len) (A C G T = 0..3, anything else 4)
+ * starting at genome position seq_start; its statistics (pos, stat)[stat_off .. + n_stat);
+ * control statistics [ctrl_off .. + n_ctrl) (tb2_accuracy_label_ctrl); the sorted unique
+ * mod / unmod locations of its (chrm, strand) inside [start, end) (tb2_accuracy_label_truth);
+ * strand 0 '+', 1 '-'.  Unused ranges are 0.  The calls take the blocks as rows of
+ * TB2_ACC_BLOCK_FIELDS int64 values in this field order. */
+typedef struct tb2_acc_block {
+    int64_t seq_off, seq_len, seq_start;
+    int64_t stat_off, n_stat, ctrl_off, n_ctrl;
+    int64_t mod_off, n_mod, unmod_off, n_unmod;
+    int64_t strand;
+} tb2_acc_block;
+#define TB2_ACC_BLOCK_FIELDS 12
+
+/* empties every slot */
+int tb2_accuracy_reset(tb2_ctx *ctx);
+/* entries of a slot */
+int tb2_accuracy_count(tb2_ctx *ctx, int slot, int64_t *n_out);
+/* a slot's entries in append order (stat, label 0/1) */
+int tb2_accuracy_download(tb2_ctx *ctx, int slot, double *stat_out, uint8_t *label_out);
+/* replaces a slot's entries (labels 0/1) */
+int tb2_accuracy_load(tb2_ctx *ctx, int slot, int64_t n, const double *stat, const uint8_t *label);
+/* _compute_motif_stats (tombo_stats.py:2406-2456) of n_blocks blocks: for each statistic
+ * and each motif in order whose mod base is window[bb], appends (stat, prefix match) to
+ * slot[m].  bb / ab are max(mod_pos) - 1 and max(len - mod_pos) over the motifs (1 .. 8).
+ * counts_out[b * n_motifs + m]: entries of block b for motif m.  A window the reference
+ * cannot index (IndexError) -> TB2_ERR_UNEXPECTED and nothing appended. */
+int tb2_accuracy_label_motif(tb2_ctx *ctx, int64_t n_blocks, const int64_t *blocks,
+                             int64_t n_seq, const uint8_t *seq, int64_t n_stat,
+                             const uint32_t *pos, const double *stat, int n_motifs,
+                             const tb2_motif *motifs, const int32_t *slot, int64_t bb,
+                             int64_t ab, int64_t *counts_out);
+/* _compute_ground_truth_stats (:2458-2483): statistics at a mod or unmod location, in block
+ * order, labelled pos in mod; counts_out[b] */
+int tb2_accuracy_label_truth(tb2_ctx *ctx, int64_t n_blocks, const int64_t *blocks,
+                             int64_t n_stat, const uint32_t *pos, const double *stat,
+                             int64_t n_mod, const int64_t *mod_locs, int64_t n_unmod,
+                             const int64_t *unmod_locs, int slot, int64_t *counts_out);
+/* _compute_ctrl_motif_stats (:2485-2535): per block and motif, the re.finditer sites of the
+ * motif ('+') or its reverse complement ('-') in reg_seq; sample statistics at a site
+ * (True), then control statistics at a site (False); counts_out[b * n_motifs + m] */
+int tb2_accuracy_label_ctrl(tb2_ctx *ctx, int64_t n_blocks, const int64_t *blocks,
+                            int64_t n_seq, const uint8_t *seq, int64_t n_stat,
+                            const uint32_t *pos, const double *stat, int64_t n_ctrl,
+                            const uint32_t *ctrl_pos, const double *ctrl_stat, int n_motifs,
+                            const tb2_motif *motifs, const int32_t *slot, int64_t *counts_out);
+/* prep_accuracy_rates of one slot: the labels in Python's (stat, label) tuple order, then
+ * compute_accuracy_rates sampled at rate_idx (tp_rate, fp_rate) and prec_idx (precision),
+ * n_points each, computed by the caller as numpy's linspace(...).astype(int64).  An empty
+ * slot or a NaN statistic -> TB2_ERR_INVALID_ARG; a buffer that does not fit on the device
+ * -> TB2_ERR_CAPACITY.  tb2_last_timing out[0] is the kernel time. */
+int tb2_accuracy_curve(tb2_ctx *ctx, int slot, int64_t n_points, const int64_t *rate_idx,
+                       const int64_t *prec_idx, double *tp_rate, double *fp_rate,
+                       double *precision);
+/* compute_accuracy_rates (:2384-2404) of n labels already in order */
+int tb2_accuracy_rates_ordered(tb2_ctx *ctx, int64_t n, const uint8_t *labels, int64_t n_points,
+                               const int64_t *rate_idx, const int64_t *prec_idx,
+                               double *tp_rate, double *fp_rate, double *precision);
 
 #ifdef __cplusplus
 }

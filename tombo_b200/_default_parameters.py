@@ -57,3 +57,4 @@ KERNEL_DENSITY_RANGE = (-5, 5)             # :150
 ALT_EST_PCTL = 5                           # :151
 NUM_DENS_POINTS = 500                      # :164
 NUM_READS_TO_ADJUST_MODEL = 5000           # :174
+ROC_PLOT_POINTS = 1000                     # :181

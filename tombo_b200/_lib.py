@@ -45,6 +45,13 @@ class Policy(C.Structure):
                 ('subsample_seed', C.c_uint32), ('rescue', C.c_uint32)]
 
 
+# tb2_acc_block: one statistics block of an accuracy labelling call, passed as a row of
+# TB2_ACC_BLOCK_FIELDS int64 values
+ACC_BLOCK_DTYPE = np.dtype([(name, np.int64) for name in (
+    'seq_off', 'seq_len', 'seq_start', 'stat_off', 'n_stat', 'ctrl_off', 'n_ctrl', 'mod_off',
+    'n_mod', 'unmod_off', 'n_unmod', 'strand')])
+
+
 class Motif(C.Structure):
     """tb2_motif: a TomboMotif as IUPAC bit sets (A = 1, C = 2, G = 4, T = 8)"""
     _fields_ = [('len', C.c_int32), ('mod_pos', C.c_int32), ('mask', C.c_uint8 * 32)]
@@ -66,6 +73,8 @@ def motif_struct(motif):
     return m
 
 
+TB2_ERR_UNEXPECTED, TB2_ERR_INVALID_ARG = 100, 201
+
 _lib = None
 _lock = threading.Lock()
 
@@ -75,6 +84,7 @@ _I, _CTX = C.c_int, C.c_void_p
 pI, pI32, pI64, pF64 = P(C.c_int), P(C.c_int32), P(i64), P(f64)
 pI8, pU8 = P(C.c_int8), P(C.c_uint8)
 pPar, pPol, pSV, pMotif = P(Params), P(Policy), P(ScaleValues), P(Motif)
+pU32 = P(C.c_uint32)
 _PROTOS = {
     'tb2_abi_version': (_I, []),
     'tb2_device_count': (_I, []),
@@ -149,6 +159,18 @@ _PROTOS = {
     'tb2_kernel_densities': (_I, [_CTX, i64, pF64, pI64, i64, pF64, f64, pF64, pF64, pF64]),
     'tb2_kmer_level_summaries': (_I, [_CTX, i64, i64, pF64, pI64, pI64, i64, _I, pF64, pF64, pI64]),
     'tb2_kmer_medians': (_I, [_CTX, i64, i64, pI64, pF64, pF64, pI64, pF64, pF64]),
+    'tb2_accuracy_reset': (_I, [_CTX]),
+    'tb2_accuracy_count': (_I, [_CTX, _I, pI64]),
+    'tb2_accuracy_download': (_I, [_CTX, _I, pF64, pU8]),
+    'tb2_accuracy_load': (_I, [_CTX, _I, i64, pF64, pU8]),
+    'tb2_accuracy_label_motif': (_I, [_CTX, i64, pI64, i64, pU8, i64, pU32, pF64, _I, pMotif, pI32,
+                                      i64, i64, pI64]),
+    'tb2_accuracy_label_truth': (_I, [_CTX, i64, pI64, i64, pU32, pF64, i64, pI64, i64, pI64, _I,
+                                      pI64]),
+    'tb2_accuracy_label_ctrl': (_I, [_CTX, i64, pI64, i64, pU8, i64, pU32, pF64, i64, pU32, pF64, _I,
+                                     pMotif, pI32, pI64]),
+    'tb2_accuracy_curve': (_I, [_CTX, _I, i64, pI64, pI64, pF64, pF64, pF64]),
+    'tb2_accuracy_rates_ordered': (_I, [_CTX, i64, pU8, i64, pI64, pI64, pF64, pF64, pF64]),
 }
 
 
@@ -875,6 +897,116 @@ class Context(object):
             self.handle, n, keys.shape[0], ptr(keys, i64), ptr(levels, f64), ptr(sds, f64),
             ptr(cnt, i64), ptr(med_lv, f64), ptr(med_sd, f64)))
         return cnt, med_lv, med_sd
+
+    # accuracy of modified-base calls (csrc/accuracy.cu).  ``blocks`` is an ACC_BLOCK_DTYPE
+    # array, ``seq`` the blocks' sequence codes, ``pos`` / ``stat`` their statistics.
+    def _blocks(self, blocks):
+        blocks = np.ascontiguousarray(blocks, dtype=ACC_BLOCK_DTYPE)
+        return blocks, blocks.ctypes.data_as(pI64)
+
+    def _label_args(self, pos, stat):
+        pos = np.ascontiguousarray(pos, dtype=np.uint32)
+        stat = as_f64(stat)
+        if pos.shape != stat.shape:
+            raise ValueError('pos and stat need one entry per statistic')
+        return pos, stat
+
+    def accuracy_reset(self):
+        self.check(self.lib.tb2_accuracy_reset(self.handle))
+
+    def accuracy_count(self, slot):
+        n = i64(0)
+        self.check(self.lib.tb2_accuracy_count(self.handle, int(slot), C.byref(n)))
+        return int(n.value)
+
+    def accuracy_download(self, slot):
+        """(stats f64, labels bool) of a slot in append order"""
+        n = self.accuracy_count(slot)
+        st, lab = np.empty(max(1, n)), np.empty(max(1, n), dtype=np.uint8)
+        self.check(self.lib.tb2_accuracy_download(self.handle, int(slot), ptr(st, f64),
+                                                  ptr(lab, C.c_uint8)))
+        return st[:n], lab[:n].view(bool)
+
+    def accuracy_load(self, slot, stat, label):
+        stat = as_f64(stat)
+        label = np.ascontiguousarray(label, dtype=bool).view(np.uint8)
+        if stat.shape != label.shape:
+            raise ValueError('stat and label need the same length')
+        self.check(self.lib.tb2_accuracy_load(self.handle, int(slot), stat.shape[0],
+                                              ptr(stat, f64), ptr(label, C.c_uint8)))
+
+    def accuracy_label_motif(self, blocks, seq, pos, stat, motifs, slots, bb, ab):
+        """tb2_accuracy_label_motif -> counts (n_blocks, n_motifs)"""
+        blocks, pb = self._blocks(blocks)
+        seq = np.ascontiguousarray(seq, dtype=np.uint8)
+        pos, stat = self._label_args(pos, stat)
+        ms = (Motif * len(motifs))(*motifs)
+        sl = np.ascontiguousarray(slots, dtype=np.int32)
+        cnt = np.zeros((max(1, blocks.shape[0]), len(motifs)), dtype=np.int64)
+        rc = self.lib.tb2_accuracy_label_motif(
+            self.handle, blocks.shape[0], pb, seq.shape[0], ptr(seq, C.c_uint8), pos.shape[0],
+            ptr(pos, C.c_uint32), ptr(stat, f64), len(motifs), ms, ptr(sl, C.c_int32), int(bb),
+            int(ab), ptr(cnt, i64))
+        if rc == TB2_ERR_UNEXPECTED:
+            # a window the reference slices empty or too short: window[bb] raises there
+            raise IndexError('string index out of range')
+        self.check(rc)
+        return cnt[:blocks.shape[0]]
+
+    def accuracy_label_truth(self, blocks, pos, stat, mod_locs, unmod_locs, slot=0):
+        """tb2_accuracy_label_truth -> counts per block"""
+        blocks, pb = self._blocks(blocks)
+        pos, stat = self._label_args(pos, stat)
+        mod_locs, unmod_locs = as_i64(mod_locs), as_i64(unmod_locs)
+        cnt = np.zeros(max(1, blocks.shape[0]), dtype=np.int64)
+        self.check(self.lib.tb2_accuracy_label_truth(
+            self.handle, blocks.shape[0], pb, pos.shape[0], ptr(pos, C.c_uint32), ptr(stat, f64),
+            mod_locs.shape[0], ptr(mod_locs, i64), unmod_locs.shape[0], ptr(unmod_locs, i64),
+            int(slot), ptr(cnt, i64)))
+        return cnt[:blocks.shape[0]]
+
+    def accuracy_label_ctrl(self, blocks, seq, pos, stat, ctrl_pos, ctrl_stat, motifs, slots):
+        """tb2_accuracy_label_ctrl -> counts (n_blocks, n_motifs)"""
+        blocks, pb = self._blocks(blocks)
+        seq = np.ascontiguousarray(seq, dtype=np.uint8)
+        pos, stat = self._label_args(pos, stat)
+        ctrl_pos, ctrl_stat = self._label_args(ctrl_pos, ctrl_stat)
+        ms = (Motif * len(motifs))(*motifs)
+        sl = np.ascontiguousarray(slots, dtype=np.int32)
+        cnt = np.zeros((max(1, blocks.shape[0]), len(motifs)), dtype=np.int64)
+        self.check(self.lib.tb2_accuracy_label_ctrl(
+            self.handle, blocks.shape[0], pb, seq.shape[0], ptr(seq, C.c_uint8), pos.shape[0],
+            ptr(pos, C.c_uint32), ptr(stat, f64), ctrl_pos.shape[0], ptr(ctrl_pos, C.c_uint32),
+            ptr(ctrl_stat, f64), len(motifs), ms, ptr(sl, C.c_int32), ptr(cnt, i64)))
+        return cnt[:blocks.shape[0]]
+
+    def accuracy_curve(self, slot, rate_idx, prec_idx):
+        """tb2_accuracy_curve -> (tp_rate, fp_rate, precision)"""
+        rate_idx, prec_idx = as_i64(rate_idx), as_i64(prec_idx)
+        if rate_idx.shape != prec_idx.shape:
+            raise ValueError('rate_idx and prec_idx need the same length')
+        n = rate_idx.shape[0]
+        tp, fp, prec = np.empty(n), np.empty(n), np.empty(n)
+        rc = self.lib.tb2_accuracy_curve(
+            self.handle, int(slot), n, ptr(rate_idx, i64), ptr(prec_idx, i64), ptr(tp, f64),
+            ptr(fp, f64), ptr(prec, f64))
+        if rc == TB2_ERR_INVALID_ARG and self.lib.tb2_last_error(self.handle) == b'NaN statistic':
+            raise ValueError('NaN statistic: the order of the statistics is undefined')
+        self.check(rc)
+        return tp, fp, prec
+
+    def accuracy_rates_ordered(self, labels, rate_idx, prec_idx):
+        """tb2_accuracy_rates_ordered -> (tp_rate, fp_rate, precision)"""
+        labels = np.ascontiguousarray(labels, dtype=bool).view(np.uint8)
+        rate_idx, prec_idx = as_i64(rate_idx), as_i64(prec_idx)
+        if rate_idx.shape != prec_idx.shape:
+            raise ValueError('rate_idx and prec_idx need the same length')
+        n = rate_idx.shape[0]
+        tp, fp, prec = np.empty(n), np.empty(n), np.empty(n)
+        self.check(self.lib.tb2_accuracy_rates_ordered(
+            self.handle, labels.shape[0], ptr(labels, C.c_uint8), n, ptr(rate_idx, i64),
+            ptr(prec_idx, i64), ptr(tp, f64), ptr(fp, f64), ptr(prec, f64)))
+        return tp, fp, prec
 
 
 def make_policy(kind='DNA', outlier_thresh=5.0, max_raw_cpts=200,

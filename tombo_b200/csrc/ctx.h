@@ -58,6 +58,7 @@ struct GroupState;       // group_stats.cu
 struct DebugState;       // debug.cu
 struct KdeState;         // model_est.cu
 struct KmerModelState;   // kmer_model.cu
+struct AccuracyState;    // accuracy.cu
 
 struct tb2_ctx {
     int device = 0;
@@ -79,6 +80,7 @@ struct tb2_ctx {
     std::shared_ptr<DebugState> debug;
     std::shared_ptr<KdeState> kde;
     std::shared_ptr<KmerModelState> kmer;
+    std::shared_ptr<AccuracyState> accuracy;
     // tb2_resquiggle_batch pipelines large batches over two lanes (child contexts with
     // their own stream and buffers): H2D of chunk k+1 overlaps the kernels of chunk k
     std::vector<tb2_ctx *> lanes;

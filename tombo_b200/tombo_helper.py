@@ -19,7 +19,7 @@ __all__ = [
     'TomboError', 'readData', 'TomboMotif', 'resquiggleParams', 'startClipParams',
     'stallParams', 'resquiggleResults', 'alignInfo', 'genomeLocation', 'sequenceData',
     'channelInfo', 'dpResults', 'scaleValues', 'seqSampleType', 'regionStats', 'groupStats',
-    'get_seq_kmers', 'rev_comp', 'warning_message', 'parse_locs_file',
+    'get_seq_kmers', 'rev_comp', 'warning_message', 'parse_locs_file', 'parse_motif_descs',
     'valid_cpts_w_cap', 'valid_cpts_w_cap_t_test', 'banded_traceback',
     'adaptive_banded_forward_pass', 'get_raw_read_slot', 'get_multiple_slots_read_centric']
 
@@ -255,6 +255,23 @@ def parse_locs_file(locs_fn):
                 'All provided locations from {} were incorrectly formatted. ' +
                 'Ensure that provided file is in BED format.').format(locs_fn))
     return dict((cs, np.array(sorted(cs_poss))) for cs, cs_poss in raw_locs.items())
+
+
+def parse_motif_descs(stat_motif_descs):
+    """tombo_helper.py:710-730: ``"motif:mod_pos:name[::motif2:mod_pos2:name2...]"`` -> a list
+    of ``(TomboMotif, name)``; a malformed description raises TomboError where the reference
+    exits"""
+    parsed_motif_descs = []
+    try:
+        for motif_desc in stat_motif_descs.split('::'):
+            raw_motif, mod_pos, mod_name = motif_desc.split(':')
+            motif = TomboMotif(raw_motif, int(mod_pos))
+            parsed_motif_descs.append((motif, mod_name))
+    except Exception:
+        raise TomboError(
+            'Invalid motif decriptions format. Format descriptions as: ' +
+            '"motif:mod_pos:name[::motif2:mod_pos2:name2...]".')
+    return parsed_motif_descs
 
 
 # ---- native wrappers (tombo_helper.py:76-102) -> CUDA -----------------------------

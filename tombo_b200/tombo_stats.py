@@ -20,7 +20,7 @@ from ._default_parameters import (
     MIN_EVENT_TO_SEQ_RATIO, OCLLHR_SCALE, OCLLHR_HEIGHT, OCLLHR_POWER, STALL_PARAMS,
     FM_OFFSET_DEFAULT, SMALLEST_PVAL, MEAN_PRIOR_CONST, SD_PRIOR_CONST, ALT_EST_BATCH,
     MAX_KMER_OBS, MIN_KMER_OBS_TO_EST, NUM_READS_TO_ADJUST_MODEL, COLLAPSE_RNA_STALLS,
-    USE_RNA_EVENT_SCALE, OUTLIER_THRESH)
+    USE_RNA_EVENT_SCALE, OUTLIER_THRESH, ROC_PLOT_POINTS)
 
 __all__ = [
     'TomboModel', 'AltModel', 'normalize_raw_signal', 'compute_base_means',
@@ -35,7 +35,8 @@ __all__ = [
     'parse_kmer_densities_file', 'isolate_alt_density', 'extract_kmer_levels',
     'tabulate_kmer_levels', 'tabulate_mod_kmer_levels', 'center_model_to_median_norm',
     'estimate_kmer_model', 'estimate_motif_alt_model', 'compute_de_novo_reads_stats',
-    'compute_sample_compare_reads_stats', 'compute_reg_stats']
+    'compute_sample_compare_reads_stats', 'compute_reg_stats', 'compute_accuracy_rates',
+    'compute_auc', 'compute_mean_avg_precison', 'prep_accuracy_rates', 'accuracy_curves']
 
 # E|N(0,1)| = sqrt(2 / pi); the reference evaluates scipy.stats.halfnorm.expect()
 # (tombo_stats.py:84), which returns this value (SURVEY.md 8c-2)
@@ -1644,3 +1645,299 @@ def estimate_motif_alt_model(reads_index, motif_desc, upstrm_bases, dnstrm_bases
                        alt_base=motif.mod_base, motif=motif)
     alt_ref._make_constant_sd()
     return alt_ref
+
+
+# ---- accuracy of modified-base calls (tombo plot roc and friends) ---------------------
+# Labelling runs on the device (csrc/accuracy.cu) into one slot per modification name; the
+# drop-ins download the slots as the reference's (stat, bool) lists, accuracy_curves turns
+# them into curves where they lie.
+_SEQ_CODE = np.full(256, 4, dtype=np.uint8)
+for _b, _c in _CODE.items():
+    _SEQ_CODE[ord(_b)] = _c
+
+
+def _seq_codes(seq):
+    """reg_seq -> codes (A C G T = 0..3, anything else 4, which no motif class matches)"""
+    return _SEQ_CODE[np.frombuffer(seq.encode('latin-1', 'replace'), dtype=np.uint8)]
+
+
+def _motif_setup(motif_descs):
+    """(mod names in first-seen order, slot per motif, tb2_motif per motif, bb, ab)"""
+    names = list(dict.fromkeys(name for _, name in motif_descs))
+    slots = [names.index(name) for _, name in motif_descs]
+    if len(motif_descs) > 8 or len(names) > 16:
+        raise th.TomboError('At most 8 motifs and 16 modification names per call.')
+    motifs = [_lib.motif_struct(m) for m, _ in motif_descs]
+    bb = max(m.mod_pos for m, _ in motif_descs) - 1
+    ab = max(m.motif_len - m.mod_pos for m, _ in motif_descs)
+    return names, slots, motifs, bb, ab
+
+
+def _reg_seq_bounds(strand, start, end, bb, ab):
+    if strand == '+':
+        return max(start - bb, 0), end + ab
+    return max(start - ab, 0), end + bb
+
+
+def _window_raises(pos, seq_start, seq_len, strand, bb, ab):
+    """does window[bb] raise IndexError in _compute_motif_stats for some statistic (the uint32
+    slice start wraps, or the clipped window is at most bb long)"""
+    r = pos.astype(np.int64) - seq_start
+    lo, hi = (r - bb, r + ab + 1) if strand == '+' else (r - ab, r + bb + 1)
+    return bool(np.any((lo < 0) | (np.minimum(hi, seq_len) - lo <= bb)))
+
+
+class _Blocks(object):
+    """statistics blocks of one labelling call laid out for the device"""
+
+    def __init__(self):
+        self.desc, self.seq, self.pos, self.stat, self.cpos, self.cstat = [], [], [], [], [], []
+        self.n_seq = self.n_stat = self.n_ctrl = 0
+
+    def add(self, strand, pos, stat, codes=None, seq_start=0, cpos=None, cstat=None, loc_ranges=None):
+        d = np.zeros((), dtype=_lib.ACC_BLOCK_DTYPE)
+        d['strand'] = 0 if strand == '+' else 1
+        d['stat_off'], d['n_stat'] = self.n_stat, pos.shape[0]
+        self.pos.append(pos.astype(np.uint32))
+        self.stat.append(np.asarray(stat, dtype=np.float64))
+        self.n_stat += pos.shape[0]
+        if codes is not None:
+            d['seq_off'], d['seq_len'], d['seq_start'] = self.n_seq, codes.shape[0], seq_start
+            self.seq.append(codes)
+            self.n_seq += codes.shape[0]
+        if cpos is not None:
+            d['ctrl_off'], d['n_ctrl'] = self.n_ctrl, cpos.shape[0]
+            self.cpos.append(cpos.astype(np.uint32))
+            self.cstat.append(np.asarray(cstat, dtype=np.float64))
+            self.n_ctrl += cpos.shape[0]
+        if loc_ranges is not None:
+            d['mod_off'], d['n_mod'], d['unmod_off'], d['n_unmod'] = loc_ranges
+        self.desc.append(d)
+
+    def __len__(self):
+        return len(self.desc)
+
+    @staticmethod
+    def _cat(parts, dtype):
+        return np.concatenate(parts) if parts else np.zeros(0, dtype=dtype)
+
+    def arrays(self):
+        blocks = np.array(self.desc, dtype=_lib.ACC_BLOCK_DTYPE)
+        return (blocks, self._cat(self.seq, np.uint8), self._cat(self.pos, np.uint32),
+                self._cat(self.stat, np.float64), self._cat(self.cpos, np.uint32),
+                self._cat(self.cstat, np.float64))
+
+
+def _label_motif(ctx, stats, motif_descs, genome_index, stats_per_block, total_stats_limit):
+    """_compute_motif_stats into the context's slots -> mod names"""
+    names, slots, motifs, bb, ab = _motif_setup(motif_descs)
+    slot_name = stats._stat_slot
+    blocks = _Blocks()
+    total_num_stats = 0
+    for chrm, strand, start, end, block_stats in stats:
+        seq_start, seq_end = _reg_seq_bounds(strand, start, end, bb, ab)
+        reg_seq = genome_index.get_seq(chrm, seq_start, seq_end, error_end=False)
+        if stats_per_block is not None and block_stats.shape[0] > stats_per_block:
+            block_stats = block_stats[np.random.choice(
+                block_stats.shape[0], stats_per_block, replace=False)]
+        total_num_stats += block_stats.shape[0]
+        codes = _seq_codes(reg_seq)
+        pos = block_stats['pos']
+        blocks.add(strand, pos, block_stats[slot_name], codes, int(seq_start))
+        # the reference raises in this block and pulls no further one
+        if _window_raises(pos, int(seq_start), codes.shape[0], strand, bb, ab):
+            break
+        if total_stats_limit is not None and total_num_stats >= total_stats_limit:
+            break
+    ctx.accuracy_reset()
+    if len(blocks):
+        b, seq, pos, st, _, _ = blocks.arrays()
+        ctx.accuracy_label_motif(b, seq, pos, st, motifs, slots, bb, ab)
+    return names
+
+
+def _sorted_locs(locs):
+    """{(chrm, strand): locations} -> ({key: (offset, sorted unique int64)}, concatenation)"""
+    out, parts, off = {}, [], 0
+    for key, v in locs.items():
+        u = np.unique(np.asarray(v).astype(np.int64))
+        out[key] = (off, u)
+        parts.append(u)
+        off += u.shape[0]
+    return out, (np.concatenate(parts) if parts else np.zeros(0, dtype=np.int64))
+
+
+def _loc_range(table, key, start, end):
+    if key not in table:
+        return 0, 0
+    off, u = table[key]
+    lo, hi = np.searchsorted(u, [start, end], side='left')
+    return off + int(lo), int(hi - lo)
+
+
+def _label_truth(ctx, stats, ground_truth_locs):
+    """_compute_ground_truth_stats into slot 0 -> [mod name]"""
+    mod_locs, unmod_locs, mod_name = ground_truth_locs
+    mod_tab, mod_all = _sorted_locs(mod_locs)
+    unmod_tab, unmod_all = _sorted_locs(unmod_locs)
+    slot_name = stats._stat_slot
+    blocks = _Blocks()
+    for chrm, strand, start, end, block_stats in stats:
+        ranges = (_loc_range(mod_tab, (chrm, strand), start, end) +
+                  _loc_range(unmod_tab, (chrm, strand), start, end))
+        blocks.add(strand, block_stats['pos'], block_stats[slot_name], loc_ranges=ranges)
+    ctx.accuracy_reset()
+    if len(blocks):
+        b, _, pos, st, _, _ = blocks.arrays()
+        ctx.accuracy_label_truth(b, pos, st, mod_all, unmod_all, 0)
+    return [mod_name]
+
+
+def _label_ctrl(ctx, stats, ctrl_stats, motif_descs, genome_index, total_stats_limit):
+    """_compute_ctrl_motif_stats into the context's slots -> mod names.  With a limit, each
+    block is labelled before the next one is pulled, as the reference counts appended entries."""
+    names, slots, motifs, bb, ab = _motif_setup(motif_descs)
+    slot_name = stats._stat_slot
+    ctx.accuracy_reset()
+    blocks = _Blocks()
+    empty = np.zeros(0, dtype=np.uint32)
+
+    def flush(blocks):
+        if not len(blocks):
+            return 0
+        b, seq, pos, st, cpos, cst = blocks.arrays()
+        return int(ctx.accuracy_label_ctrl(b, seq, pos, st, cpos, cst, motifs, slots).sum())
+
+    total_num_stats = 0
+    for chrm, strand, start, end, block_stats in stats:
+        seq_start, seq_end = _reg_seq_bounds(strand, start, end, bb, ab)
+        reg_seq = genome_index.get_seq(chrm, seq_start, seq_end, error_end=False)
+        ctrl_block_stats = ctrl_stats.get_reg_stats(chrm, strand, start, end)
+        if ctrl_block_stats is None:
+            cpos, cst = empty, np.zeros(0)
+        else:
+            cpos, cst = ctrl_block_stats['pos'], ctrl_block_stats[slot_name]
+        blocks.add(strand, block_stats['pos'], block_stats[slot_name], _seq_codes(reg_seq),
+                   int(seq_start), cpos, cst)
+        if total_stats_limit is not None:
+            total_num_stats += flush(blocks)
+            blocks = _Blocks()
+            if total_num_stats >= total_stats_limit:
+                break
+    flush(blocks)
+    return names
+
+
+def _slot_tuples(ctx, names):
+    out = {}
+    for k, name in enumerate(names):
+        st, lab = ctx.accuracy_download(k)
+        out[name] = list(zip(st.tolist(), lab.tolist()))
+    return out
+
+
+def _compute_motif_stats(stats, motif_descs, genome_index, stats_per_block=None,
+                         total_stats_limit=None, device=0):
+    """tombo_stats.py:2406-2456 -> {mod name: [(stat, motif matches)]}; a window the
+    reference cannot index raises IndexError as it does"""
+    ctx = _lib.get_context(device)
+    names = _label_motif(ctx, stats, motif_descs, genome_index, stats_per_block,
+                         total_stats_limit)
+    return _slot_tuples(ctx, names)
+
+
+def _compute_ground_truth_stats(stats, ground_truth_locs, device=0):
+    """tombo_stats.py:2458-2483 -> {mod name: [(stat, pos is a mod location)]}"""
+    ctx = _lib.get_context(device)
+    return _slot_tuples(ctx, _label_truth(ctx, stats, ground_truth_locs))
+
+
+def _compute_ctrl_motif_stats(stats, ctrl_stats, motif_descs, genome_index, stats_per_block=None,
+                              total_stats_limit=None, device=0):
+    """tombo_stats.py:2485-2535 -> {mod name: [(stat, sample (True) or control (False))]};
+    ``stats_per_block`` is accepted and ignored, as in the reference"""
+    ctx = _lib.get_context(device)
+    return _slot_tuples(ctx, _label_ctrl(ctx, stats, ctrl_stats, motif_descs, genome_index,
+                                         total_stats_limit))
+
+
+def compute_auc(tp_rate, fp_rate):
+    """tombo_stats.py:2377-2378"""
+    return np.sum(tp_rate[:-1] * (fp_rate[1:] - fp_rate[:-1]))
+
+
+def compute_mean_avg_precison(tp_rate, precision):
+    """tombo_stats.py:2380-2382"""
+    return np.sum(np.diff(np.concatenate([[0, ], tp_rate, [1, ]]), ) *
+                  np.concatenate([[0, ], precision, [1, ]])[:-1])
+
+
+def _sample_idx(n, num_plot_points):
+    """the reference's sample indices: rates at linspace(0, n - 1, P), precision at
+    linspace(0, n - 1, P + 1)[1:], truncated to int64"""
+    rate_idx = np.linspace(0, n - 1, num_plot_points).astype(np.int64)
+    prec_idx = np.linspace(0, n - 1, num_plot_points + 1).astype(np.int64)[1:]
+    return rate_idx, prec_idx
+
+
+def compute_accuracy_rates(stat_has_mod, num_plot_points=ROC_PLOT_POINTS, device=0):
+    """tombo_stats.py:2384-2404: labels in statistic order -> (tp_rate, fp_rate, precision)
+    at ``num_plot_points`` points; an empty input raises IndexError as the reference does"""
+    labels = np.asarray(stat_has_mod, dtype=bool).reshape(-1)
+    if labels.shape[0] == 0:
+        raise IndexError('index -1 is out of bounds for axis 0 with size 0')
+    rate_idx, prec_idx = _sample_idx(labels.shape[0], num_plot_points)
+    return _lib.get_context(device).accuracy_rates_ordered(labels, rate_idx, prec_idx)
+
+
+def _slot_curve(ctx, slot, num_plot_points):
+    n = ctx.accuracy_count(slot)
+    rate_idx, prec_idx = _sample_idx(n, num_plot_points)
+    try:
+        tp, fp, prec = ctx.accuracy_curve(slot, rate_idx, prec_idx)
+    except ValueError as e:
+        raise th.TomboError(str(e))
+    return tp, fp, prec, compute_auc(tp, fp), compute_mean_avg_precison(tp, prec)
+
+
+def prep_accuracy_rates(all_motif_stats, device=0):
+    """_plot_commands.py:60-82 without the verbose table: {mod name: [(stat, bool)]} ->
+    (tp_rates, fp_rates, precisions, mod_names) over every name in order.  The (stat, label)
+    tuples are ordered on the device; a name without statistics raises IndexError as the
+    reference does, and a NaN statistic raises TomboError."""
+    ctx = _lib.get_context(device)
+    tp_rates, fp_rates, precisions, mod_names_for_r = [], [], [], []
+    for mod_name, mod_stats in all_motif_stats.items():
+        if len(mod_stats) == 0:
+            raise IndexError('list index out of range')
+        st = np.fromiter((x[0] for x in mod_stats), dtype=np.float64, count=len(mod_stats))
+        lab = np.fromiter((bool(x[1]) for x in mod_stats), dtype=bool, count=len(mod_stats))
+        ctx.accuracy_load(0, st, lab)
+        tp, fp, prec, _, _ = _slot_curve(ctx, 0, ROC_PLOT_POINTS)
+        tp_rates.extend(tp)
+        fp_rates.extend(fp)
+        precisions.extend(prec)
+        mod_names_for_r.extend(itertools.repeat(mod_name, len(tp)))
+    return tp_rates, fp_rates, precisions, mod_names_for_r
+
+
+def accuracy_curves(stats, motif_descs=None, genome_index=None, ground_truth_locs=None,
+                    ctrl_stats=None, stats_per_block=None, total_stats_limit=None,
+                    num_plot_points=ROC_PLOT_POINTS, device=0):
+    """Labelling and curves in one pass, with the labelled statistics kept on the device:
+    ``ground_truth_locs`` selects _compute_ground_truth_stats, else ``ctrl_stats``
+    _compute_ctrl_motif_stats, else _compute_motif_stats.  Returns {mod name: (tp_rate,
+    fp_rate, precision, auc, mean_ap)}, or None for a name without statistics; each curve
+    equals prep_accuracy_rates of the matching _compute_* result."""
+    ctx = _lib.get_context(device)
+    if ground_truth_locs is not None:
+        names = _label_truth(ctx, stats, ground_truth_locs)
+    elif ctrl_stats is not None:
+        names = _label_ctrl(ctx, stats, ctrl_stats, motif_descs, genome_index, total_stats_limit)
+    else:
+        names = _label_motif(ctx, stats, motif_descs, genome_index, stats_per_block,
+                             total_stats_limit)
+    out = {}
+    for k, name in enumerate(names):
+        out[name] = _slot_curve(ctx, k, num_plot_points) if ctx.accuracy_count(k) else None
+    return out
