@@ -261,7 +261,16 @@ int tb2_resolve_skipped_bases_with_raw(
  *   norm_signal     optional (NULL to skip): clipped, re-normalised signal with
  *                   the raw offsets; read r holds segs_r[-1] valid samples.
  * flags bit0: norm_params_changed after the last iteration, bit1: rescued with
- * save params, bit2: static (short read) path taken. */
+ * save params, bit2: static (short read) path taken (clear for a read that failed
+ * before the alignment).
+ * A sequence without a k-mer (fewer than kmer_width codes) fails with
+ * TB2_ERR_TOO_MUCH_SIGNAL as in resquiggle_read, or TB2_ERR_DISCORDANT_LEN when the read
+ * has too few samples for one event.
+ * raw_off[0] and seq_off[0] must be 0 and neither may decrease (else
+ * TB2_ERR_INVALID_ARG), whether the batch goes as one chunk or is pipelined.
+ * Whatever it returns, the call leaves no resident batch: afterwards the calls on the
+ * resident batch (tb2_batch_download, tb2_batch_alt_llr, tb2_batch_alt_llr_motif,
+ * tb2_batch_de_novo_region) return TB2_ERR_INVALID_ARG until the next tb2_batch_compute. */
 int tb2_resquiggle_batch(
     tb2_ctx *ctx, int64_t n_reads, const void *raw, int raw_dtype,
     const int64_t *raw_off, const uint8_t *seq, const int64_t *seq_off,

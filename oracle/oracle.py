@@ -448,11 +448,11 @@ def levels_from_codes(codes, means, sds, k):
 
 
 def run_batch(raw, raw_off, seq, seq_off, means, sds, k, params, save_params, pol,
-              indices=None, threads=None):
+              indices=None, threads=None, want_norm=False):
     """orc_run_read over reads `indices` of a flat batch (the C-ABI layout), on a thread
     pool (ctypes releases the GIL; oracle.c keeps no state between calls).  read_index =
     position in the batch, which keys the Theil-Sen sub-sampling like the library does.
-    Returns {index: result dict}."""
+    want_norm adds each successful read's 'norm_signal'.  Returns {index: result dict}."""
     import os
     from multiprocessing.pool import ThreadPool
     lib()
@@ -469,7 +469,8 @@ def run_batch(raw, raw_off, seq, seq_off, means, sds, k, params, save_params, po
     def one(i):
         rm, rs = levels_from_codes(seq[seq_off[i]:seq_off[i + 1]], means, sds, k)
         r = np.asarray(raw[raw_off[i]:raw_off[i + 1]], dtype=np.float64)
-        return i, run_read(r, rm, rs, params, save_params, pol, read_index=i)
+        return i, run_read(r, rm, rs, params, save_params, pol, read_index=i,
+                           want_norm=want_norm)
     if threads == 1:
         return dict(one(i) for i in indices)
     with ThreadPool(threads) as tp:

@@ -136,12 +136,18 @@ def test_large_batch_pipelined_chunks_match_single_chunk(ctx, dna_model, RPcls):
     next chunk overlaps compute); results must equal the unchunked staged path"""
     from tombo_b200 import _lib, synthetic as syn
     import bench
+    import torch
     kmer_ref, cpos = dna_model
     means, sds = syn.kmer_table(kmer_ref)
     ctx.set_model(means, sds, 6, cpos)
-    n = 4 * 132 * 32 * 2 + 1234           # > 6 x 32 reads per SM: 3 chunks on a 132-SM H100
-    raw, raw_off, codes, seq_off = syn.make_read_batch(kmer_ref, n, 60, 77)
-    # a few long reads so that the keyed sub-sampling (global read index) is exercised
+    u = torch.cuda.get_device_properties(0).multi_processor_count * 32
+    n = 8 * u + 1234                      # > 6 U reads (U = SMs x 32): chunks of 2 U, 4 U, rest
+    nb = np.full(n, 60)
+    # a few long reads (> 1000 bases) in every chunk after the first, so that the keyed
+    # Theil-Sen sub-sampling is exercised with a chunk's non-zero global read index
+    long_at = [2 * u, 2 * u + 5, 4 * u, 6 * u, 6 * u + 777, n - 1]
+    nb[long_at] = [1100, 1400, 1250, 1333, 1200, 1150]
+    raw, raw_off, codes, seq_off = syn.make_read_batch(kmer_ref, n, nb, 77)
     rp, sp = RPcls(bench.ALN_DNA), RPcls(bench.ALN_DNA, save=True)
     pol = _lib.make_policy('DNA', subsample_seed=5)
     a = ctx.resquiggle_batch(raw, raw_off, codes, seq_off, rp, sp, pol)
@@ -155,3 +161,4 @@ def test_large_batch_pipelined_chunks_match_single_chunk(ctx, dna_model, RPcls):
     assert np.array_equal(a['sig_match_score'], b['sig_match_score'], equal_nan=True)
     assert np.array_equal(a['norm_mean'], b['norm_mean'], equal_nan=True)
     assert (a['status'] == 0).mean() > 0.9
+    assert (a['status'][long_at] == 0).all()

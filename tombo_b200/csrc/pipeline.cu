@@ -486,6 +486,10 @@ static int batch_compute_impl(tb2_ctx *ctx, const tb2_params *params,
     h->has_norm_sig = want_norm_signal != 0;
     double *norm_mean_dev = h->out_norm_mean.as<double>();
     if ((rc = tb2_launch_prep(ctx, v, h->raw_in.p, h->raw_dtype, sp.is_rna, hb.total_s, hb.total_b))) return rc;
+    // k_align writes a read's first debug word (0 = static band) when it aligns the read;
+    // a read that fails before the alignment keeps -1, so flags bit 2 never shows the word
+    // of another batch that used these buffers before
+    TB2_CUDA_TRY(ctx, cudaMemsetAsync(h->buf.dbg.p, 0xff, (size_t)n * 3 * 4, s));
     if (sp.is_rna && !h->has_stalls_in && (rc = tb2_launch_stalls(ctx, v))) return rc;
     const size_t rawdp_cap = (size_t)1 << 15;
     double ms_dp = 0, dp_reads = 0;
@@ -646,13 +650,34 @@ static int resquiggle_batch_impl(tb2_ctx *ctx, int64_t n_reads, const void *raw,
                                     double *norm_mean, double *norm_signal, int32_t *status,
                                     int32_t *n_iters, int32_t *flags)
 {
-    if (n_reads == 0) return tb2_use(ctx);
     int rc = tb2_use(ctx);
     if (rc) return rc;
+    // whatever the call returns, it leaves no resident batch: the unchunked branch computes
+    // in ctx's own holder and the pipelined one in the lanes', so the resident calls
+    // (tb2_batch_alt_llr, tb2_batch_download, ...) must not see either batch afterwards
+    struct ClearResident {
+        BatchHolder *h;
+        ~ClearResident() { h->uploaded = h->computed = false; }
+    } clear_resident{holder_of(ctx)};
+    if (n_reads == 0) return TB2_OK;
     if (!raw_off || !seq_off || !params || !policy || !raw || !seq || !segs ||
         !read_start_rel_to_raw || !scale_out || !sig_match_score || !status || !n_iters || !flags ||
-        (raw_dtype != 0 && raw_dtype != 1) || n_reads > 0x7ffffff0)
+        (raw_dtype != 0 && raw_dtype != 1) || n_reads < 0 || n_reads > 0x7ffffff0)
         return TB2_ERR_INVALID_ARG;
+    if (ctx->kmer_width <= 0) { ctx->err = "tb2_set_model has not been called"; return TB2_ERR_INVALID_ARG; }
+    // the offsets are checked once for the whole batch, before the chunk schedule: the
+    // pipelined branch re-bases every chunk to 0, so its own uploads cannot see a bad start
+    if (raw_off[0] != 0 || seq_off[0] != 0) {
+        ctx->err = "raw_off[0] or seq_off[0] is not 0";
+        return TB2_ERR_INVALID_ARG;
+    }
+    for (int64_t r = 0; r < n_reads; ++r) {
+        const int64_t s = raw_off[r + 1] - raw_off[r], q = seq_off[r + 1] - seq_off[r];
+        if (s < 0 || q < 0 || s > 0x3fffffff || q - (ctx->kmer_width - 1) > 0x3fffffff) {
+            ctx->err = "raw_off or seq_off decreases, or a read holds more than 2^30 samples or bases";
+            return TB2_ERR_INVALID_ARG;
+        }
+    }
     const std::vector<int64_t> cstart = pipeline_chunk_starts(ctx->sm_count, n_reads);
     if (cstart.size() <= 2) {
         rc = tb2_batch_upload(ctx, n_reads, raw, raw_dtype, raw_off, seq, seq_off, params, policy);

@@ -46,7 +46,8 @@ k_prep(BatchView b, const T *raw, int is_rna, const double *kmeans, const double
         memset(&s, 0, sizeof(s));
         s.status = TB2_OK;
         if (n <= 0) s.status = TB2_ERR_NO_RAW;
-        if (nb <= 0 || (int)(b.seq_off[r + 1] - so) != nb + K - 1) s.status = TB2_ERR_DISCORDANT_LEN;
+        // a sequence without a k-mer (nb clamped to 0) is judged by k_begin_call, which
+        // tests the signal against the mapped bases first as resquiggle_read does
         if (any_bad) s.status = TB2_ERR_INVALID_SEQ;
         s.done = (s.status != TB2_OK);
         b.st[r] = s;
@@ -85,10 +86,15 @@ __global__ void k_begin_call(BatchView b, tb2_params p, StagePolicy pol)
     if (!rd_active(s)) return;
     const int n = (int)(b.raw_off[r + 1] - b.raw_off[r]);
     const int nb = (int)(b.base_off[r + 1] - b.base_off[r]);
+    // num_mapped_bases = len(genome_seq) - kmer_width + 1: below 1 for a sequence without a
+    // k-mer, where nb is clamped to 0
+    const long long nmb = (b.seq_off[r + 1] - b.seq_off[r]) - (b.kmer_width - 1);
     const long long a = (long long)n / p.mean_obs_per_event;
-    const long long c = (long long)((double)nb * pol.min_event_to_seq_ratio);
+    const long long c = (long long)((double)nmb * pol.min_event_to_seq_ratio);
     const long long ne = a > c ? a : c;
-    if ((double)ne / (double)p.bandwidth > (double)nb) { s.status = TB2_ERR_TOO_MUCH_SIGNAL; return; }
+    if ((double)ne / (double)p.bandwidth > (double)nmb) { s.status = TB2_ERR_TOO_MUCH_SIGNAL; return; }
+    // no k-mer and too little signal for one event: nothing to align
+    if (nb <= 0) { s.status = TB2_ERR_DISCORDANT_LEN; return; }
     if (ne > b.ev_off[r + 1] - b.ev_off[r] || ne < 2) { s.status = TB2_ERR_CAPACITY; return; }
     s.num_events = (int)ne;
 }
