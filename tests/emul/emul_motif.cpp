@@ -1,12 +1,23 @@
 // emul_motif.cpp -- TEST INFRASTRUCTURE ONLY: the motif LLR kernel's device source
 // (tombo_b200/csrc/motif_llr.cuh) run on the host through tests/emul/cuda_emul.h, the way
-// tb2_alt_model_llr_motif_batch launches it (count pass, scan, fill pass).
+// tb2_alt_model_llr_motif_batch launches it (count pass, scan, fill pass), and the offsets
+// kernel of that scan (k_scan_offsets, csrc/common.cuh).
 #include "cuda_emul.h"
 #include "../../include/tombo_b200.h"
 #include "../../tombo_b200/csrc/motif_llr.cuh"
 #include <vector>
 
 extern "C" {
+
+// k_scan_offsets over n counts of type int (u64 = 0) or unsigned long long (u64 = 1); cnt may
+// be off itself
+void emul_scan_offsets(int u64, const void *cnt, long long *off, long long n)
+{
+    emul::launch(emul::Idx3{1, 1, 1}, 1024, 0, [&]() {
+        if (u64) k_scan_offsets((const unsigned long long *)cnt, off, n);
+        else k_scan_offsets((const int *)cnt, off, n);
+    });
+}
 
 int emul_motif_can_overlap(const unsigned char *mask, int len) { return motif_can_overlap(mask, len) ? 1 : 0; }
 

@@ -1,5 +1,5 @@
-"""ctypes driver of tests/emul/libemul_motif.so: the motif LLR kernel's device source run on
-the host (TEST INFRASTRUCTURE ONLY -- see cuda_emul.h)."""
+"""ctypes driver of tests/emul/libemul_motif.so: the motif LLR kernel's and the offsets
+kernel's device source run on the host (TEST INFRASTRUCTURE ONLY -- see cuda_emul.h)."""
 import ctypes as C
 import os
 import subprocess
@@ -18,7 +18,8 @@ def lib():
     if _LIB is None:
         import tempfile
         srcs = [os.path.join(HERE, f) for f in ('emul_motif.cpp', 'cuda_emul.cpp', 'cuda_emul.h')]
-        srcs += [os.path.join(CSRC, 'motif_llr.cuh'), os.path.join(REPO, 'include', 'tombo_b200.h')]
+        srcs += [os.path.join(CSRC, f) for f in os.listdir(CSRC) if f.endswith(('.cuh', '.h'))]
+        srcs.append(os.path.join(REPO, 'include', 'tombo_b200.h'))
         out_dir = HERE if os.access(HERE, os.W_OK) else tempfile.mkdtemp(prefix='emul_motif_')
         so = os.path.join(out_dir, 'libemul_motif.so')
         if not os.path.exists(so) or any(os.path.getmtime(s) > os.path.getmtime(so) for s in srcs):
@@ -60,3 +61,22 @@ def llr_motif(norm_mean, mean_off, seq, seq_off, read_start, strand, K, cpos, km
         i64(reg_end), _p(llr, f64), _p(pos, i64), _p(off, i64), _p(st, C.c_int32))
     t = int(off[-1])
     return llr[:t], pos[:t], off, st[:n]
+
+
+def scan_offsets(cnt, in_place=False):
+    """k_scan_offsets on the host: int32 or uint64 counts -> int64 offsets (n + 1).  in_place
+    (uint64 only) scans a buffer of n + 1 entries that holds the counts, as accuracy does."""
+    cnt = np.ascontiguousarray(cnt)
+    n = cnt.shape[0]
+    u64 = cnt.dtype == np.uint64
+    assert u64 or cnt.dtype == np.int32
+    if in_place:
+        assert u64
+        buf = np.zeros(n + 1, dtype=np.uint64)
+        buf[:n] = cnt
+        lib().emul_scan_offsets(C.c_int(1), _p(buf, C.c_uint64), _p(buf, C.c_longlong), C.c_longlong(n))
+        return buf.view(np.int64)
+    off = np.full(n + 1, -1, dtype=np.int64)
+    lib().emul_scan_offsets(C.c_int(1 if u64 else 0), _p(cnt, C.c_uint64 if u64 else C.c_int32),
+                            _p(off, C.c_longlong), C.c_longlong(n))
+    return off

@@ -166,7 +166,7 @@ def test_single_base_motif_matches_existing_entry_on_llr_goldens(ctx, RPcls, gna
             assert np.array_equal(new[0], g[key])
 
 
-# 3. seeded sweep over more than one k_scan_sites chunk
+# 3. seeded sweep over more than one k_scan_offsets chunk
 @pytest.mark.parametrize('raw,mod_pos,base', mc.MOTIFS)
 def test_seeded_sweep_matches_restatement(ctx, raw, mod_pos, base):
     kmer_ref, K, cpos, kmeans, ksds, alt = _set(ctx, 'DNA', base)

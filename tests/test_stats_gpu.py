@@ -147,7 +147,7 @@ def test_host_array_calls_reject_counts_past_int_max(ctx, call):
 
 
 # ---------------------------------------------------------------------------
-# tb2_batch_alt_llr on a resident batch of >= 2 500 reads (three k_scan_sites chunks)
+# tb2_batch_alt_llr on a resident batch of >= 2 500 reads (three k_scan_offsets chunks)
 # ---------------------------------------------------------------------------
 def test_resident_llr_over_three_scan_chunks(ctx, RPcls):
     from tombo_b200 import _lib, synthetic as syn

@@ -175,25 +175,6 @@ __global__ void __launch_bounds__(AT) k_acc_count(AccArgs a, long long *cnt, int
     if (tid < nm) cnt[(size_t)b * nm + tid] = (long long)sh[tid];
 }
 
-// exclusive block scan of one value per thread; returns the prefix, *total the sum
-__device__ __forceinline__ unsigned int block_excl(unsigned int x, unsigned int *warp_tot, unsigned int &total)
-{
-    const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
-    unsigned int inc = x;
-#pragma unroll
-    for (int off = 1; off < 32; off <<= 1) {
-        const unsigned int o = __shfl_up_sync(0xffffffffu, inc, off);
-        if (lane >= off) inc += o;
-    }
-    __syncthreads();
-    if (lane == 31) warp_tot[warp] = inc;
-    __syncthreads();
-    unsigned int before = 0;
-    total = 0;
-    for (int q = 0; q < AT / 32; ++q) { if (q < warp) before += warp_tot[q]; total += warp_tot[q]; }
-    return before + inc - x;
-}
-
 // scatter pass of one slot (motifs `mask`): block b's entries go to out[off[b] ...] in the
 // reference's append order
 template <int MODE>
@@ -233,7 +214,9 @@ k_acc_scatter(AccArgs a, unsigned int mask, const long long *off, double *out_st
             }
         }
         unsigned int total;
-        long long o = base + block_excl(c, warp_tot, total);
+        __syncthreads();          // here rather than after the fills: a warp's fills overlap the next lookups
+        long long o = base + tb2_block_excl_scan<AT>(c, warp_tot, total);
+        base += total;
         if (c) {
             if (MODE == MODE_MOTIF) {
                 for (int m = 0; m < a.n_motifs; ++m) {
@@ -249,7 +232,6 @@ k_acc_scatter(AccArgs a, unsigned int mask, const long long *off, double *out_st
                 out_lab[o] = (unsigned char)lab;
             }
         }
-        base += total;
     }
 }
 
@@ -379,9 +361,10 @@ k_acc_tile_scan(const unsigned int *th, long long n_tiles, const unsigned long l
         const long long t = t0 + threadIdx.x;
         const unsigned int x = t < n_tiles ? row[t] : 0;
         unsigned int total;
-        const unsigned int ex = block_excl(x, warp_tot, total);
-        if (t < n_tiles) orow[t] = base + ex;
+        __syncthreads();
+        const unsigned long long o = base + tb2_block_excl_scan<AT>(x, warp_tot, total);
         base += total;
+        if (t < n_tiles) orow[t] = o;
     }
 }
 
@@ -436,34 +419,8 @@ __global__ void __launch_bounds__(AT) k_acc_lab_tiles(const unsigned char *lab, 
         if (i < n) s += lab[i];
     }
     unsigned int total;
-    block_excl(s, warp_tot, total);
+    tb2_block_excl_scan<AT>(s, warp_tot, total);
     if (threadIdx.x == 0) tsum[t] = total;
-}
-
-// exclusive scan of the tile sums in place (one block); tsum[n_tiles] = the total
-__global__ void __launch_bounds__(AT) k_acc_scan_tiles(unsigned long long *tsum, long long n_tiles)
-{
-    __shared__ unsigned long long warp_tot[AT / 32];
-    const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
-    unsigned long long base = 0;
-    for (long long t0 = 0; t0 < n_tiles; t0 += AT) {
-        const long long t = t0 + threadIdx.x;
-        const unsigned long long x = t < n_tiles ? tsum[t] : 0;
-        unsigned long long inc = x;
-#pragma unroll
-        for (int off = 1; off < 32; off <<= 1) {
-            const unsigned long long o = __shfl_up_sync(0xffffffffu, inc, off);
-            if (lane >= off) inc += o;
-        }
-        __syncthreads();
-        if (lane == 31) warp_tot[warp] = inc;
-        __syncthreads();
-        unsigned long long before = 0, total = 0;
-        for (int q = 0; q < AT / 32; ++q) { if (q < warp) before += warp_tot[q]; total += warp_tot[q]; }
-        if (t < n_tiles) tsum[t] = base + before + inc - x;
-        base += total;
-    }
-    if (threadIdx.x == 0) tsum[n_tiles] = base;
 }
 
 // tp_cumsum at index q: one warp per query
@@ -704,7 +661,7 @@ int rates(tb2_ctx *ctx, const unsigned char *lab, long long n, long long n_point
     TB2_CUDA_TRY(ctx, cudaMemcpyAsync(idx + n_points, pidx, (size_t)n_points * 8, cudaMemcpyHostToDevice, q));
     k_acc_lab_tiles<<<(unsigned)n_tiles, AT, 0, q>>>(lab, n, tsum);
     TB2_CHECK_LAUNCH(ctx);
-    k_acc_scan_tiles<<<1, AT, 0, q>>>(tsum, n_tiles);
+    k_scan_offsets<<<1, 1024, 0, q>>>(tsum, (long long *)tsum, n_tiles);   // in place
     TB2_CHECK_LAUNCH(ctx);
     const long long threads = 2 * n_points * 32;
     k_acc_rates<<<(unsigned)((threads + AT - 1) / AT), AT, 0, q>>>(lab, tsum, n_tiles, n, idx, idx + n_points,

@@ -28,6 +28,49 @@ __device__ __forceinline__ double tb2_neg_inf()
 
 __device__ __forceinline__ int tb2_lane() { return threadIdx.x & 31; }
 
+// Exclusive prefix sum over a block of NT == blockDim.x threads, each giving one value:
+// returns the sum of v over the lower thread indices and sets total to the block's sum, in
+// every thread.  warp_tot is shared memory of NT / 32 entries.  The one barrier sits between
+// the store of the warp totals and their loads, so two calls that use the same warp_tot need
+// a barrier between them (a fast warp would otherwise overwrite totals a slow one still reads).
+template <int NT, class T>
+__device__ __forceinline__ T tb2_block_excl_scan(T v, T *warp_tot, T &total)
+{
+    static_assert(NT % 32 == 0 && NT <= 1024, "whole warps, one block");
+    const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+    T inc = v;
+#pragma unroll
+    for (int off = 1; off < 32; off <<= 1) {
+        const T o = __shfl_up_sync(TB2_FULL_MASK, inc, off);
+        if (lane >= off) inc += o;
+    }
+    if (lane == 31) warp_tot[warp] = inc;
+    __syncthreads();
+    T before = 0;
+    total = 0;
+    for (int q = 0; q < NT / 32; ++q) { if (q < warp) before += warp_tot[q]; total += warp_tot[q]; }
+    return before + inc - v;
+}
+
+// off[i] = cnt[0] + .. + cnt[i - 1] for 0 <= i <= n (off[0] = 0, off[n] the total), as one
+// block of 1024 threads.  cnt may alias off (a scan in place): off[i] is written only by the
+// thread that read cnt[i], after the barrier that follows every read of the chunk.
+template <class T>
+__global__ void __launch_bounds__(1024) k_scan_offsets(const T *cnt, long long *off, long long n)
+{
+    __shared__ long long warp_tot[32];
+    long long base = 0;
+    for (long long c0 = 0; c0 < n; c0 += 1024) {
+        const long long i = c0 + threadIdx.x;
+        long long total;
+        const long long o = base + tb2_block_excl_scan<1024>(i < n ? (long long)cnt[i] : 0LL, warp_tot, total);
+        base += total;
+        if (i < n) off[i] = o;
+        __syncthreads();
+    }
+    if (threadIdx.x == 0) off[n] = base;
+}
+
 // Correctly rounded a / b for a divisor b that is reused (one k-mer level SD per DP
 // row).  Once per divisor: y = RN(1/b) (__drcp_rn), e = 1 - b*y (exact in one FMA) and
 // ylo = RN(e*y), so that y + ylo = (1/b)(1 + eps), |eps| <= 2 u^2.  Per quotient four

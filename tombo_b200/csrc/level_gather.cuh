@@ -65,7 +65,9 @@ __device__ bool keep_at(const int *cs, const int *cc, long long p, long long n, 
     return l + r - 1 >= min_run;
 }
 
-// exclusive scan over a 1024-thread block; `tot` gets the block total
+// exclusive scan over a 1024-thread block; `tot` gets the block total.  k_compact keeps this
+// two-level form rather than tb2_block_excl_scan (common.cuh): there every thread reads all 32
+// warp totals, which for four 64-bit scans per chunk made k_compact ~40 us slower per call.
 __device__ __forceinline__ long long block_scan(long long v, long long *ws, long long &tot)
 {
     const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;

@@ -45,19 +45,10 @@ k_llr(LlrArgs a, int *counts, const long long *site_off, double *llr_out, long l
     const int i0 = min(testable, tid * per), i1 = min(testable, i0 + per);
     unsigned int mine = 0;
     for (int i = i0; i < i1; ++i) mine += (bases[i + K - 1] == a.alt_code);
-    const int lane = tid & 31, warp = tid >> 5;
-    unsigned int inc = mine;
-#pragma unroll
-    for (int off = 1; off < 32; off <<= 1) {
-        const unsigned int o = __shfl_up_sync(0xffffffffu, inc, off);
-        if (lane >= off) inc += o;
-    }
-    if (lane == 31) warp_tot[warp] = inc;
-    __syncthreads();
-    unsigned int base = 0, total = 0;
-    for (int q = 0; q < 8; ++q) { if (q < warp) base += warp_tot[q]; total += warp_tot[q]; }
+    unsigned int total;
+    const unsigned int before = tb2_block_excl_scan<256>(mine, warp_tot, total);
     if (!FILL) { if (tid == 0) counts[r] = (int)total; return; }
-    long long o = site_off[r] + base + inc - mine;
+    long long o = site_off[r] + before;
     for (int i = i0; i < i1; ++i) {
         if (bases[i + K - 1] != a.alt_code) continue;
         // alt_pos = i: k-mers i .. i+K-1 of the trimmed sequence, means' = means[cpos + .]
@@ -79,33 +70,6 @@ __global__ void k_mean_stds(const double *sig, const long long *segs, long long 
     means[i] = m;
     for (long long k = a; k < z; ++k) { const double d = sig[k] - m; v += d * d; }
     sds[i] = sqrt(v / (double)(z - a));
-}
-
-// exclusive scan of the per-read site counts (one block; n is a batch, <= ~1e6)
-__global__ void __launch_bounds__(1024) k_scan_sites(const int *cnt, long long *site_off, int n)
-{
-    __shared__ long long warp_tot[32];
-    __shared__ long long base_s;
-    const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
-    if (tid == 0) { base_s = 0; site_off[0] = 0; }
-    __syncthreads();
-    for (int c0 = 0; c0 < n; c0 += 1024) {
-        const int i = c0 + tid;
-        long long v = i < n ? cnt[i] : 0, inc = v;
-#pragma unroll
-        for (int off = 1; off < 32; off <<= 1) {
-            const long long o = __shfl_up_sync(0xffffffffu, inc, off);
-            if (lane >= off) inc += o;
-        }
-        if (lane == 31) warp_tot[warp] = inc;
-        __syncthreads();
-        long long before = 0, total = 0;
-        for (int q = 0; q < 32; ++q) { if (q < warp) before += warp_tot[q]; total += warp_tot[q]; }
-        if (i < n) site_off[i + 1] = base_s + before + inc;
-        __syncthreads();
-        if (tid == 0) base_s += total;
-        __syncthreads();
-    }
 }
 }  // namespace
 
@@ -177,7 +141,7 @@ int run_llr(tb2_ctx *ctx, LlrKernel<A> count, LlrKernel<A> fill, const A &a, int
     TB2_CUDA_TRY(ctx, pos.reserve(max_sites * 8 + 8));
     count<<<n, 256, 0, s>>>(a, P[L_CNT].as<int>(), nullptr, nullptr, nullptr);
     TB2_CHECK_LAUNCH(ctx);
-    k_scan_sites<<<1, 1024, 0, s>>>(P[L_CNT].as<int>(), site_off.as<long long>(), n);
+    k_scan_offsets<<<1, 1024, 0, s>>>(P[L_CNT].as<int>(), site_off.as<long long>(), n);
     TB2_CHECK_LAUNCH(ctx);
     fill<<<n, 256, 0, s>>>(a, nullptr, site_off.as<long long>(), llr.as<double>(), pos.as<long long>());
     TB2_CHECK_LAUNCH(ctx);

@@ -4,6 +4,7 @@
 // (TomboMotif tombo_helper.py:542-640), both strands and region clipping.  Included by
 // llr.cu and, for the host emulation, by tests/emul/emul_motif.cpp.
 #pragma once
+#include "common.cuh"
 
 struct LlrArgs {
     int n_reads, K, cpos, alt_code, use_std;
@@ -173,18 +174,10 @@ k_llr_motif(MotifArgs a, int *counts, const long long *site_off, double *llr_out
         const int i0 = min(n, tid * per), i1 = min(n, i0 + per);
         unsigned int mine = 0;
         for (int i = i0; i < i1; ++i) mine += motif_at(a.m, bases, nb, g.s0 + i);
-        unsigned int inc = mine;
-#pragma unroll
-        for (int off = 1; off < 32; off <<= 1) {
-            const unsigned int o = __shfl_up_sync(0xffffffffu, inc, off);
-            if (lane >= off) inc += o;
-        }
-        if (lane == 31) warp_tot[warp] = inc;
-        __syncthreads();
-        unsigned int before = 0, total = 0;
-        for (int q = 0; q < 8; ++q) { if (q < warp) before += warp_tot[q]; total += warp_tot[q]; }
+        unsigned int total;
+        const unsigned int before = tb2_block_excl_scan<256>(mine, warp_tot, total);
         if (!FILL) { if (tid == 0) counts[r] = (int)total; return; }
-        long long o = site_off[r] + before + inc - mine;
+        long long o = site_off[r] + before;
         for (int i = i0; i < i1; ++i) {
             if (!motif_at(a.m, bases, nb, g.s0 + i)) continue;
             llr_out[o] = llr_site(a.s, tb, tm, i);

@@ -21,6 +21,7 @@
 //         tb2_region_stats_add_tests.
 #include "batch.h"
 #include "kernels.h"
+#include "common.cuh"
 #include "fisher.cuh"
 #include <cmath>
 #include <cstring>
@@ -77,25 +78,15 @@ k_region_finalize(const int *cnt, long long reg_start, long long reg_len, double
                   long long *cov_out, long long *valid_out, long long *n_out)
 {
     __shared__ int warp_tot[32];
-    __shared__ long long base_s;
-    const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
-    if (tid == 0) base_s = 0;
-    __syncthreads();
+    const int tid = threadIdx.x;
+    long long base = 0;
     for (long long c0 = 0; c0 < reg_len; c0 += 1024) {
         const long long p = c0 + tid;
         const int cov = p < reg_len ? cnt[p] : 0;
         const int has = cov > 0;
-        int inc = has;
-#pragma unroll
-        for (int off = 1; off < 32; off <<= 1) {
-            const int o = __shfl_up_sync(0xffffffffu, inc, off);
-            if (lane >= off) inc += o;
-        }
-        if (lane == 31) warp_tot[warp] = inc;
-        __syncthreads();
-        int before = 0, total = 0;
-        for (int q = 0; q < 32; ++q) { if (q < warp) before += warp_tot[q]; total += warp_tot[q]; }
-        const long long o = base_s + before + inc - has;
+        int total;
+        const long long o = base + tb2_block_excl_scan<1024>(has, warp_tot, total);
+        base += total;
         if (has && o < cap) {
             const int valid = cnt[reg_len + p], ge = cnt[2 * reg_len + p];
             // np.greater_equal(...).sum() / base_stats.shape[0], NaN on empty (:4114-4118)
@@ -109,10 +100,8 @@ k_region_finalize(const int *cnt, long long reg_start, long long reg_len, double
                                        : (rint(frac * (double)valid) + unmod) / ((double)valid + (unmod + mod));
         }
         __syncthreads();
-        if (tid == 0) base_s += total;
-        __syncthreads();
     }
-    if (tid == 0) *n_out = base_s;
+    if (tid == 0) *n_out = base;
 }
 
 
@@ -207,8 +196,7 @@ k_compare_compact(const CompareRead *rd, const double *m, const double *rm, cons
                   double *stat_out, long long *pos_out)
 {
     __shared__ int warp_tot[8];
-    __shared__ int base_s;
-    const int r = blockIdx.x, tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
+    const int r = blockIdx.x, tid = threadIdx.x;
     const CompareRead d = rd[r];
     if (!FILL) {
         int st = TB2_OK;
@@ -224,60 +212,24 @@ k_compare_compact(const CompareRead *rd, const double *m, const double *rm, cons
     } else if (d.skip || status[r] != TB2_OK) {
         return;
     }
-    if (tid == 0) base_s = 0;
-    __syncthreads();
+    if (FILL) { stat_out += stat_off[r]; pos_out += stat_off[r]; }
+    int base = 0;
     for (int c0 = 0; c0 < d.n; c0 += 256) {
         const int i = c0 + tid;
         const double v = i < d.n ? fout[d.seg0 + i] : NAN;
         const int keep = !isnan(v);
-        int inc = keep;
-#pragma unroll
-        for (int off = 1; off < 32; off <<= 1) {
-            const int o = __shfl_up_sync(0xffffffffu, inc, off);
-            if (lane >= off) inc += o;
-        }
-        if (lane == 31) warp_tot[warp] = inc;
-        __syncthreads();
-        int before = 0, total = 0;
-        for (int q = 0; q < 8; ++q) { if (q < warp) before += warp_tot[q]; total += warp_tot[q]; }
+        int total;
+        const int o = base + tb2_block_excl_scan<256>(keep, warp_tot, total);
+        base += total;
         if (FILL && keep) {
-            const long long o = stat_off[r] + base_s + before + inc - keep;
             stat_out[o] = v;
             pos_out[o] = d.gstart + i;
         }
         __syncthreads();
-        if (tid == 0) base_s += total;
-        __syncthreads();
     }
-    if (!FILL && tid == 0) cnt[r] = base_s;
+    if (!FILL && tid == 0) cnt[r] = base;
 }
 
-// exclusive scan of per-read counts into stat_off (n + 1 entries); one block
-__global__ void __launch_bounds__(1024) k_scan_counts(const int *cnt, long long *stat_off, int n)
-{
-    __shared__ long long warp_tot[32];
-    __shared__ long long base_s;
-    const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
-    if (tid == 0) { base_s = 0; stat_off[0] = 0; }
-    __syncthreads();
-    for (int c0 = 0; c0 < n; c0 += 1024) {
-        const int i = c0 + tid;
-        long long inc = i < n ? cnt[i] : 0;
-#pragma unroll
-        for (int off = 1; off < 32; off <<= 1) {
-            const long long o = __shfl_up_sync(0xffffffffu, inc, off);
-            if (lane >= off) inc += o;
-        }
-        if (lane == 31) warp_tot[warp] = inc;
-        __syncthreads();
-        long long before = 0, total = 0;
-        for (int q = 0; q < 32; ++q) { if (q < warp) before += warp_tot[q]; total += warp_tot[q]; }
-        if (i < n) stat_off[i + 1] = base_s + before + inc;
-        __syncthreads();
-        if (tid == 0) base_s += total;
-        __syncthreads();
-    }
-}
 }  // namespace
 
 // ---------------------------------------------------------------------------
@@ -733,7 +685,7 @@ extern "C" int tb2_sample_compare_region_stats(tb2_ctx *ctx, int64_t n_reads, co
     k_compare_compact<false><<<n, 256, 0, s>>>(drd, a.means, a.rm, a.rs, a.out, a.lag, cnt, st,
                                                nullptr, nullptr, nullptr);
     TB2_CHECK_LAUNCH(ctx);
-    k_scan_counts<<<1, 1024, 0, s>>>(cnt, soff, n);
+    k_scan_offsets<<<1, 1024, 0, s>>>(cnt, soff, n);
     TB2_CHECK_LAUNCH(ctx);
     k_compare_compact<true><<<n, 256, 0, s>>>(drd, a.means, a.rm, a.rs, a.out, a.lag, nullptr, st,
                                               soff, R.tests_stat.as<double>(), R.tests_pos.as<long long>());

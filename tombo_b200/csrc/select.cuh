@@ -132,21 +132,11 @@ __device__ unsigned long long tb2_block_select_key(F f, Pred pred, int n, int k,
             }
         }
         __syncthreads();
-        // inclusive scan of the 256 bins (thread t <-> bin t)
+        // exclusive scan of the 256 bins (thread t <-> bin t)
         const unsigned int h = sm.hist[tid];
-        unsigned int inc = h;
-        const int lane = tid & 31, warp = tid >> 5;
-#pragma unroll
-        for (int off = 1; off < 32; off <<= 1) {
-            const unsigned int o = __shfl_up_sync(TB2_FULL_MASK, inc, off);
-            if (lane >= off) inc += o;
-        }
-        if (lane == 31) sm.warp_tot[warp] = inc;
-        __syncthreads();
-        unsigned int base = 0;
-        for (int w = 0; w < warp; ++w) base += sm.warp_tot[w];
-        inc += base;
-        const unsigned int exc = inc - h;
+        unsigned int total;
+        const unsigned int exc = tb2_block_excl_scan<TB2_SEL_THREADS>(h, sm.warp_tot, total);
+        const unsigned int inc = exc + h;
         if (h > 0 && exc <= kk && kk < inc) { sm.sel_bin = tid; sm.sel_below = exc; sm.sel_cnt = h; }
         __syncthreads();
         prefix |= (unsigned long long)sm.sel_bin << shift;

@@ -465,17 +465,8 @@ k_cpts(BatchView b, tb2_params p, int on_raw, int smem_words)
     const int w0 = min(nw, tid * per), w1 = min(nw, w0 + per);
     unsigned int mine = 0;
     for (int wd = w0; wd < w1; ++wd) mine += __popc(K[wd]);
-    unsigned int inc = mine;
-#pragma unroll
-    for (int off = 1; off < 32; off <<= 1) {
-        const unsigned int o = __shfl_up_sync(TB2_FULL_MASK, inc, off);
-        if (lane >= off) inc += o;
-    }
-    if (lane == 31) sm.warp_tot[warp] = inc;
-    __syncthreads();
-    unsigned int base = 0, total = 0;
-    for (int q = 0; q < ST_THREADS / 32; ++q) { if (q < warp) base += sm.warp_tot[q]; total += sm.warp_tot[q]; }
-    unsigned int o = base + inc - mine;
+    unsigned int total;
+    unsigned int o = tb2_block_excl_scan<ST_THREADS>(mine, sm.warp_tot, total);
     int *cp = b.cpts + b.ev_off[r];
     for (int wd = w0; wd < w1; ++wd) {
         uint32_t kw = K[wd];
@@ -1269,19 +1260,9 @@ k_theil_sen(BatchView b, StagePolicy pol, int first_call)
             __syncthreads();
             const int per = (TS_SBINS + 2 + ST_THREADS - 1) / ST_THREADS;
             const int q0 = min(TS_SBINS + 2, tid * per), q1 = min(TS_SBINS + 2, q0 + per);
-            unsigned int mine = 0;
+            unsigned int mine = 0, total;
             for (int q = q0; q < q1; ++q) mine += t.hist[q];
-            const int lane = tid & 31, warp = tid >> 5;
-            unsigned int inc = mine;
-#pragma unroll
-            for (int off = 1; off < 32; off <<= 1) {
-                const unsigned int o = __shfl_up_sync(TB2_FULL_MASK, inc, off);
-                if (lane >= off) inc += o;
-            }
-            if (lane == 31) sm.warp_tot[warp] = inc;
-            __syncthreads();
-            unsigned int run = inc - mine;
-            for (int q = 0; q < warp; ++q) run += sm.warp_tot[q];
+            unsigned int run = tb2_block_excl_scan<ST_THREADS>(mine, sm.warp_tot, total);
             for (int q = q0; q < q1; ++q) { run += t.hist[q]; t.hist[q] = run; }   // cum[q]: samples in bins <= q
             __syncthreads();
         }
@@ -1463,20 +1444,9 @@ k_theil_sen(BatchView b, StagePolicy pol, int first_call)
                     // bins holding the sampled ranks kA and kB: 256 threads x 17 bins
                     const int per = (TS_ABINS + 2 + ST_THREADS - 1) / ST_THREADS;
                     const int q0 = min(TS_ABINS + 2, tid * per), q1 = min(TS_ABINS + 2, q0 + per);
-                    unsigned int mine = 0;
+                    unsigned int mine = 0, total;
                     for (int q = q0; q < q1; ++q) mine += t.hist[q];
-                    const int lane = tid & 31, warp = tid >> 5;
-                    unsigned int inc = mine;
-#pragma unroll
-                    for (int off = 1; off < 32; off <<= 1) {
-                        const unsigned int o = __shfl_up_sync(TB2_FULL_MASK, inc, off);
-                        if (lane >= off) inc += o;
-                    }
-                    if (lane == 31) sm.warp_tot[warp] = inc;
-                    __syncthreads();
-                    unsigned int base = 0;
-                    for (int q = 0; q < warp; ++q) base += sm.warp_tot[q];
-                    long long cum = (long long)base + inc - mine;
+                    long long cum = tb2_block_excl_scan<ST_THREADS>(mine, sm.warp_tot, total);
                     for (int q = q0; q < q1; ++q) {
                         const long long c = t.hist[q];
                         if (kA >= cum && kA < cum + c) t.b1 = q;
