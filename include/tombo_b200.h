@@ -658,6 +658,71 @@ int tb2_accuracy_rates_ordered(tb2_ctx *ctx, int64_t n, const uint8_t *labels, i
                                const int64_t *rate_idx, const int64_t *prec_idx,
                                double *tp_rate, double *fp_rate, double *precision);
 
+/* ---- statistics files (aggregate_per_read_stats, ModelStats / LevelStats writers) ---- */
+/* One per-read statistics block (chrm, strand, start, end, block_stats) of a PerReadStats
+ * iterator: its statistics (pos, stat)[stat_off .. + n_stat), its start, the id of its
+ * chromosome in the most-significant table (order of first appearance) and its strand as the
+ * byte the table stores ('+' or '-').  The calls take the blocks as rows of
+ * TB2_SF_BLOCK_FIELDS int64 values in this field order. */
+typedef struct tb2_sf_block {
+    int64_t start, stat_off, n_stat, chrm, strand;
+} tb2_sf_block;
+#define TB2_SF_BLOCK_FIELDS 5
+
+/* _agg_stats_worker (tombo_stats.py:4699-4725, apply_per_read_thresh :4084-4122) and the
+ * block table of ModelStats._write_stat_block (:2737-2773, calc_damp_fraction :2537-2552) for
+ * n_blocks blocks of region_size positions.  stat_type 0: alternative-model LLRs (|stat| >=
+ * thresh is valid when lower_thresh is NaN = None), 1: p-values.  Unlike
+ * tb2_region_stats_add, a NaN statistic is not dropped: it counts in cov, in valid_cov only
+ * for stat_type 1 without lower_thresh, and never as >= thresh.  Block b's rows are its
+ * covered positions in ascending order without those whose damp_frac is NaN; row_off
+ * (n_blocks + 1, caller's) receives their offsets.  control_cov is 0 for every row (:2756).
+ * The rows stay on the device for tb2_stats_file_aggregate_download and
+ * tb2_most_signif_add_aggregate until the next call.  A position outside [start, start +
+ * region_size), an invalid block range, region_size outside 1 .. 2^28 or a NaN threshold or
+ * pseudo-count -> TB2_ERR_INVALID_ARG; a buffer that does not fit on the device ->
+ * TB2_ERR_CAPACITY.  tb2_last_timing out[0] is the kernel time. */
+int tb2_stats_file_aggregate(tb2_ctx *ctx, int64_t n_blocks, const int64_t *blocks,
+                             int64_t region_size, int64_t n_stat, const uint32_t *pos,
+                             const double *stat, double single_read_thresh, double lower_thresh,
+                             int stat_type, double unmod_count, double mod_count,
+                             int64_t *row_off);
+/* the rows of the last aggregation (row_off[n_blocks] each, caller's buffers) */
+int tb2_stats_file_aggregate_download(tb2_ctx *ctx, uint32_t *pos_out, double *damp_frac_out,
+                                      double *frac_out, uint32_t *cov_out, uint32_t *valid_cov_out);
+
+/* The running most-significant table of ModelStats (kind 0: rows damp_frac, frac, pos, cov,
+ * control_cov, valid_cov, chrm, strand) or LevelStats (kind 1: stat, pos, cov, control_cov,
+ * chrm, strand), held on the device: after any sequence of adds it is the first
+ * num_most_signif rows of one stable sort of every row added, in order of arrival, by numpy's
+ * structured-array order (the key field, then the other fields in dtype order, floats as
+ * numbers with -0.0 == +0.0) -- what _add_to_most_signif / _update_most_signif
+ * (:2714-2735) and the trim of _close_write (:2775-2785) leave, at every
+ * most_signif_num_batches.  A context holds one table: begin opens it empty with its kind and
+ * size (1 .. 2^31 - 1), and refuses (TB2_ERR_INVALID_ARG) while one is open, so two writers
+ * open at once (one per alternative model in test_significance) need a context each; end
+ * closes it; reset empties it and keeps it open.  The other calls need an open table. */
+int tb2_most_signif_begin(tb2_ctx *ctx, int kind, int64_t num_most_signif);
+int tb2_most_signif_end(tb2_ctx *ctx);
+int tb2_most_signif_reset(tb2_ctx *ctx);
+/* n rows of one block from host arrays (regionStats / groupStats after the NaN filter of
+ * _write_stat_block): key is damp_frac or stat; frac and valid_cov are read for kind 0 only.
+ * A NaN key -> TB2_ERR_INVALID_ARG. */
+int tb2_most_signif_add_rows(tb2_ctx *ctx, int64_t n, const double *key, const double *frac,
+                             const uint32_t *pos, const uint32_t *cov, const uint32_t *control_cov,
+                             const uint32_t *valid_cov, uint32_t chrm, uint8_t strand);
+/* every row of the last tb2_stats_file_aggregate, in block order, without leaving the device
+ * (kind 0 only) */
+int tb2_most_signif_add_aggregate(tb2_ctx *ctx);
+/* rows in the table: min(num_most_signif, rows added) */
+int tb2_most_signif_count(tb2_ctx *ctx, int64_t *n_out);
+/* the table in order into caller's buffers of tb2_most_signif_count rows; frac_out and
+ * valid_cov_out are written for kind 0 only.  tb2_last_timing out[0] after count or get is the
+ * time of the sort they ran. */
+int tb2_most_signif_get(tb2_ctx *ctx, double *key_out, double *frac_out, uint32_t *pos_out,
+                        uint32_t *cov_out, uint32_t *control_cov_out, uint32_t *valid_cov_out,
+                        uint32_t *chrm_out, uint8_t *strand_out);
+
 #ifdef __cplusplus
 }
 #endif

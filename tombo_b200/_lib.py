@@ -171,6 +171,17 @@ _PROTOS = {
                                      pMotif, pI32, pI64]),
     'tb2_accuracy_curve': (_I, [_CTX, _I, i64, pI64, pI64, pF64, pF64, pF64]),
     'tb2_accuracy_rates_ordered': (_I, [_CTX, i64, pU8, i64, pI64, pI64, pF64, pF64, pF64]),
+    'tb2_stats_file_aggregate': (_I, [_CTX, i64, pI64, i64, i64, pU32, pF64, f64, f64, _I, f64, f64,
+                                      pI64]),
+    'tb2_stats_file_aggregate_download': (_I, [_CTX, pU32, pF64, pF64, pU32, pU32]),
+    'tb2_most_signif_begin': (_I, [_CTX, _I, i64]),
+    'tb2_most_signif_end': (_I, [_CTX]),
+    'tb2_most_signif_reset': (_I, [_CTX]),
+    'tb2_most_signif_add_rows': (_I, [_CTX, i64, pF64, pF64, pU32, pU32, pU32, pU32, C.c_uint32,
+                                      C.c_uint8]),
+    'tb2_most_signif_add_aggregate': (_I, [_CTX]),
+    'tb2_most_signif_count': (_I, [_CTX, pI64]),
+    'tb2_most_signif_get': (_I, [_CTX, pF64, pF64, pU32, pU32, pU32, pU32, pU32, pU8]),
 }
 
 
@@ -1007,6 +1018,91 @@ class Context(object):
             self.handle, labels.shape[0], ptr(labels, C.c_uint8), n, ptr(rate_idx, i64),
             ptr(prec_idx, i64), ptr(tp, f64), ptr(fp, f64), ptr(prec, f64)))
         return tp, fp, prec
+
+    # ---- statistics files ---------------------------------------------------
+    def stats_file_aggregate(self, blocks, region_size, pos, stat, single_read_thresh,
+                             lower_thresh, stat_type, unmod_count, mod_count):
+        """tb2_stats_file_aggregate -> row_off (n_blocks + 1); ``blocks`` rows are (start,
+        stat_off, n_stat, chrm id, strand byte).  The rows stay on the device for
+        stats_file_download and most_signif_add_aggregate."""
+        blocks = as_i64(blocks).reshape(-1, 5)
+        pos = np.ascontiguousarray(pos, dtype=np.uint32)
+        stat = as_f64(stat)
+        if pos.shape != stat.shape:
+            raise ValueError('pos and stat need the same length')
+        row_off = np.zeros(blocks.shape[0] + 1, dtype=np.int64)
+        rc = self.lib.tb2_stats_file_aggregate(
+            self.handle, blocks.shape[0], ptr(blocks, i64), int(region_size), stat.shape[0],
+            ptr(pos, C.c_uint32), ptr(stat, f64), float(single_read_thresh),
+            float('nan') if lower_thresh is None else float(lower_thresh), int(stat_type),
+            float(unmod_count), float(mod_count), ptr(row_off, i64))
+        err = self.lib.tb2_last_error(self.handle).decode() if rc == TB2_ERR_INVALID_ARG else ''
+        if err:
+            raise TomboB200Error('tb2_stats_file_aggregate: ' + err)
+        self.check(rc)
+        return row_off
+
+    def stats_file_download(self, n_rows):
+        """the last aggregation's rows: (pos u4, damp_frac, frac, cov u4, valid_cov u4)"""
+        out = (np.empty(n_rows, np.uint32), np.empty(n_rows), np.empty(n_rows),
+               np.empty(n_rows, np.uint32), np.empty(n_rows, np.uint32))
+        self.check(self.lib.tb2_stats_file_aggregate_download(
+            self.handle, ptr(out[0], C.c_uint32), ptr(out[1], f64), ptr(out[2], f64),
+            ptr(out[3], C.c_uint32), ptr(out[4], C.c_uint32)))
+        return out
+
+    def most_signif_begin(self, level, num_most_signif):
+        """open this context's table; raises while another is open"""
+        rc = self.lib.tb2_most_signif_begin(self.handle, int(bool(level)), int(num_most_signif))
+        if rc == TB2_ERR_INVALID_ARG and self.lib.tb2_last_error(self.handle):
+            raise TomboB200Error('tb2_most_signif_begin: ' + self.lib.tb2_last_error(self.handle).decode())
+        self.check(rc)
+
+    def most_signif_end(self):
+        self.check(self.lib.tb2_most_signif_end(self.handle))
+
+    def most_signif_reset(self):
+        self.check(self.lib.tb2_most_signif_reset(self.handle))
+
+    def most_signif_add_rows(self, key, pos, cov, control_cov, chrm, strand, frac=None,
+                             valid_cov=None):
+        """one block's rows; ``strand`` is the table's byte (b'+' / b'-')"""
+        key = as_f64(key)
+        n = key.shape[0]
+        u4 = [np.ascontiguousarray(a, dtype=np.uint32) for a in (pos, cov, control_cov)]
+        fr = as_f64(frac) if frac is not None else None
+        vc = np.ascontiguousarray(valid_cov, dtype=np.uint32) if valid_cov is not None else None
+        if any(a.shape[0] != n for a in u4 + [x for x in (fr, vc) if x is not None]):
+            raise ValueError('row columns need the same length')
+        sb = strand if isinstance(strand, int) else bytes(strand)[:1][0]
+        self.check(self.lib.tb2_most_signif_add_rows(
+            self.handle, n, ptr(key, f64), ptr(fr, f64) if fr is not None else None,
+            ptr(u4[0], C.c_uint32), ptr(u4[1], C.c_uint32), ptr(u4[2], C.c_uint32),
+            ptr(vc, C.c_uint32) if vc is not None else None, int(chrm), int(sb)))
+
+    def most_signif_add_aggregate(self):
+        self.check(self.lib.tb2_most_signif_add_aggregate(self.handle))
+
+    def most_signif_count(self):
+        n = i64(0)
+        self.check(self.lib.tb2_most_signif_count(self.handle, C.byref(n)))
+        return int(n.value)
+
+    def most_signif_get(self):
+        """the table in order: dict of columns (key, frac, pos, cov, control_cov, valid_cov,
+        chrm, strand as S1)"""
+        n = self.most_signif_count()
+        c = dict(key=np.empty(n), frac=np.empty(n), pos=np.empty(n, np.uint32),
+                 cov=np.empty(n, np.uint32), control_cov=np.empty(n, np.uint32),
+                 valid_cov=np.empty(n, np.uint32), chrm=np.empty(n, np.uint32),
+                 strand=np.empty(n, np.uint8))
+        self.check(self.lib.tb2_most_signif_get(
+            self.handle, ptr(c['key'], f64), ptr(c['frac'], f64), ptr(c['pos'], C.c_uint32),
+            ptr(c['cov'], C.c_uint32), ptr(c['control_cov'], C.c_uint32),
+            ptr(c['valid_cov'], C.c_uint32), ptr(c['chrm'], C.c_uint32),
+            ptr(c['strand'], C.c_uint8)))
+        c['strand'] = c['strand'].view('S1')
+        return c
 
 
 def make_policy(kind='DNA', outlier_thresh=5.0, max_raw_cpts=200,

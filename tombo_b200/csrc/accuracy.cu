@@ -19,6 +19,7 @@
 // exactly the reference's append order (DESIGN.md §3 "Accuracy of modified-base calls").
 #include "ctx.h"
 #include "motif_llr.cuh"
+#include "radix_sort.cuh"
 #include <algorithm>
 #include <cmath>
 #include <cstring>
@@ -31,8 +32,9 @@ namespace {
 constexpr int AT = 256;                 // threads per block of every accuracy kernel
 constexpr int MAXM = 8;                 // motifs per labelling call
 constexpr int MAXSLOT = 16;             // slots (modification names)
-constexpr int IPT = 16;                 // radix sort: items per thread of a tile
-constexpr int TILE = AT * IPT;
+constexpr int IPT = RADIX_IPT;          // radix sort: items per thread of a tile
+constexpr int TILE = RADIX_TILE;
+static_assert(AT == RADIX_NT, "the curve kernels share the radix sort's tiles");
 
 enum { A_BLK = 0, A_SEQ, A_POS, A_STAT, A_CPOS, A_CSTAT, A_MOD, A_UNMOD, A_SITE, A_CNT, A_OFF,
        A_KEY0, A_KEY1, A_LAB0, A_LAB1, A_THIST, A_TOFF, A_GHIST, A_IDX, A_OUT, A_COUNT };
@@ -275,16 +277,8 @@ __global__ void __launch_bounds__(AT) k_acc_sites(AccArgs a, unsigned char *site
 }
 
 // ---------------------------------------------------------------------------
-// curve: order-preserving keys, stable LSD radix sort carrying the label, rates
+// curve: order-preserving keys (radix_sort.cuh), stable LSD radix sort carrying the label, rates
 // ---------------------------------------------------------------------------
-// float64 bits -> uint64 whose unsigned order is the numeric order; -0.0 folds onto +0.0
-__device__ __forceinline__ unsigned long long order_key(double x)
-{
-    unsigned long long u = (unsigned long long)__double_as_longlong(x);
-    if (u == 0x8000000000000000ull) u = 0;
-    return (u >> 63) ? ~u : (u | 0x8000000000000000ull);
-}
-
 // keys, NaN flag, and the histograms of all eight key digits (ghist[d * 256 + v]) and of
 // the label (ghist[8 * 256 + l]); a histogram does not depend on the order, so every pass
 // that a single bin holds is known before the sort starts
@@ -314,98 +308,6 @@ __global__ void k_acc_label_hist(const unsigned char *lab, long long n, unsigned
         t += lab[i];
     t = __reduce_add_sync(0xffffffffu, t);
     if ((threadIdx.x & 31) == 0 && t) atomicAdd(ghist + 8 * 256 + 1, (unsigned long long)t);
-}
-
-// digit of one pass: shift 64 is the label pass, else 8 bits of the key
-__device__ __forceinline__ int digit_of(unsigned long long k, unsigned char l, int shift)
-{
-    return shift == 64 ? l : (int)((k >> shift) & 255u);
-}
-
-// tile histograms, digit-major: th[d * n_tiles + t]
-__global__ void __launch_bounds__(AT)
-k_acc_tile_hist(const unsigned long long *key, const unsigned char *lab, long long n, int shift,
-                unsigned int *th, long long n_tiles)
-{
-    __shared__ unsigned int h[256];
-    h[threadIdx.x] = 0;
-    __syncthreads();
-    const long long t = blockIdx.x, i0 = t * TILE;
-    for (int r = 0; r < IPT; ++r) {
-        const long long i = i0 + r * AT + threadIdx.x;
-        if (i < n) atomicAdd(h + digit_of(key[i], lab[i], shift), 1u);
-    }
-    __syncthreads();
-    th[(size_t)threadIdx.x * n_tiles + t] = h[threadIdx.x];
-}
-
-// one block per digit: toff[d * n_tiles + t] = (entries of smaller digits) + (entries of
-// digit d in tiles before t)
-__global__ void __launch_bounds__(AT)
-k_acc_tile_scan(const unsigned int *th, long long n_tiles, const unsigned long long *pass_hist,
-                unsigned long long *toff)
-{
-    __shared__ unsigned int warp_tot[AT / 32];
-    __shared__ unsigned long long base_sh;
-    const int d = blockIdx.x;
-    if (threadIdx.x == 0) {
-        unsigned long long s = 0;
-        for (int e = 0; e < d; ++e) s += pass_hist[e];
-        base_sh = s;
-    }
-    __syncthreads();
-    unsigned long long base = base_sh;
-    const unsigned int *row = th + (size_t)d * n_tiles;
-    unsigned long long *orow = toff + (size_t)d * n_tiles;
-    for (long long t0 = 0; t0 < n_tiles; t0 += AT) {
-        const long long t = t0 + threadIdx.x;
-        const unsigned int x = t < n_tiles ? row[t] : 0;
-        unsigned int total;
-        __syncthreads();
-        const unsigned long long o = base + tb2_block_excl_scan<AT>(x, warp_tot, total);
-        base += total;
-        if (t < n_tiles) orow[t] = o;
-    }
-}
-
-// stable scatter of one tile: IPT rounds of AT items in index order; within a round, an
-// item's rank among equal digits is its rank in its warp (match_any) plus the counts of the
-// same digit in earlier warps and earlier rounds
-__global__ void __launch_bounds__(AT)
-k_acc_scatter_pass(const unsigned long long *kin, const unsigned char *lin, unsigned long long *kout,
-                   unsigned char *lout, long long n, int shift, const unsigned long long *toff,
-                   long long n_tiles)
-{
-    __shared__ unsigned long long run[256];
-    __shared__ unsigned int wcnt[AT / 32][256];
-    const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
-    const long long t = blockIdx.x, i0 = t * TILE;
-    run[tid] = toff[(size_t)tid * n_tiles + t];
-    for (int w = 0; w < AT / 32; ++w) wcnt[w][tid] = 0;
-    __syncthreads();
-    for (int r = 0; r < IPT; ++r) {
-        const long long i = i0 + r * AT + tid;
-        const bool live = i < n;
-        unsigned long long k = 0;
-        unsigned char l = 0;
-        int d = 256 + lane;                              // a bin of its own for dead lanes
-        if (live) { k = kin[i]; l = lin[i]; d = digit_of(k, l, shift); }
-        const unsigned int peers = __match_any_sync(0xffffffffu, d);
-        const unsigned int rank = __popc(peers & ((1u << lane) - 1u));
-        if (live && rank == 0) wcnt[warp][d] = __popc(peers);
-        __syncthreads();
-        if (live) {
-            unsigned long long o = run[d] + rank;
-            for (int w = 0; w < warp; ++w) o += wcnt[w][d];
-            kout[o] = k;
-            lout[o] = l;
-        }
-        __syncthreads();
-        unsigned int s = 0;
-        for (int w = 0; w < AT / 32; ++w) { s += wcnt[w][tid]; wcnt[w][tid] = 0; }
-        run[tid] += s;
-        __syncthreads();
-    }
 }
 
 // per-tile label sums
@@ -878,12 +780,12 @@ extern "C" int tb2_accuracy_curve(tb2_ctx *ctx, int slot, int64_t n_points, cons
         unsigned long long *kin = P[A_KEY0 + cur].as<unsigned long long>();
         unsigned long long *kout = P[A_KEY1 - cur].as<unsigned long long>();
         unsigned char *lin = P[A_LAB0 + cur].as<unsigned char>(), *lout = P[A_LAB1 - cur].as<unsigned char>();
-        k_acc_tile_hist<<<(unsigned)n_tiles, AT, 0, q>>>(kin, lin, n, shift, P[A_THIST].as<unsigned int>(), n_tiles);
+        k_radix_tile_hist<<<(unsigned)n_tiles, AT, 0, q>>>(kin, lin, n, shift, P[A_THIST].as<unsigned int>(), n_tiles);
         TB2_CHECK_LAUNCH(ctx);
-        k_acc_tile_scan<<<256, AT, 0, q>>>(P[A_THIST].as<unsigned int>(), n_tiles, gh + d * 256,
+        k_radix_tile_scan<<<256, AT, 0, q>>>(P[A_THIST].as<unsigned int>(), n_tiles, gh + d * 256,
                                            P[A_TOFF].as<unsigned long long>());
         TB2_CHECK_LAUNCH(ctx);
-        k_acc_scatter_pass<<<(unsigned)n_tiles, AT, 0, q>>>(kin, lin, kout, lout, n, shift,
+        k_radix_scatter_pass<<<(unsigned)n_tiles, AT, 0, q>>>(kin, lin, kout, lout, n, shift,
                                                             P[A_TOFF].as<unsigned long long>(), n_tiles);
         TB2_CHECK_LAUNCH(ctx);
         cur ^= 1;

@@ -4,7 +4,9 @@
   (``TomboReads.write_index_file`` / ``_load_index_data``, tombo_helper.py:1068-1104,
   1235-1290): what ``tombo resquiggle`` leaves behind for every later command;
 * the per-read statistics blocks of a ``PerReadStats`` file (tombo_stats.py:3335-3366) and
-  the (pos, stat, read_id) table ``collate_reg_stats`` builds for them (:4136-4154).
+  the (pos, stat, read_id) table ``collate_reg_stats`` builds for them (:4136-4154);
+* the statistics file of ``ModelStats`` / ``LevelStats`` (:2594-2636, 3064-3099): its block
+  tables and its most-significant table, which the device keeps (tb2_most_signif_*).
 
 The FAST5 ``Events`` group writer is in :mod:`tombo_b200.tombo_helper`.  HDF5 objects are
 duck-typed (anything with ``create_group`` / ``create_dataset`` / ``attrs``), h5py itself is
@@ -17,11 +19,20 @@ from collections import OrderedDict, defaultdict
 
 import numpy as np
 
+from . import _lib
 from . import tombo_helper as th
 
 INDEX_SUFFIX = '.tombo.index'
 PER_READ_BLOCKS_NAME = 'Statistic_Blocks'          # tombo_stats.py:114 STAT_BLOCKS_H5_NAME
 PER_READ_DTYPE = [(str('pos'), 'u4'), (str('stat'), 'f8'), (str('read_id'), 'u4')]
+MOST_SIGNIF_NAME = 'Most_Significant_Stats'         # tombo_stats.py:115-117
+COV_DAMP_COUNTS_NAME = 'Cov_Damp_Counts'
+COV_THRESH_NAME = 'Cov_Threshold'
+MODEL_STATS_DTYPE = [(str('damp_frac'), 'f8'), (str('frac'), 'f8'), (str('pos'), 'u4'),
+                     (str('cov'), 'u4'), (str('control_cov'), 'u4'), (str('valid_cov'), 'u4')]
+LEVEL_STATS_DTYPE = [(str('stat'), 'f8'), (str('pos'), 'u4'), (str('cov'), 'u4'),
+                     (str('control_cov'), 'u4')]
+MOST_SIGNIF_EXTRA = [(str('chrm'), 'u4'), (str('strand'), 'S1')]
 
 
 def index_filename(fast5s_dir, corr_grp='RawGenomeCorrected_000'):
@@ -145,3 +156,151 @@ class PerReadStatsWriter(object):
         if hasattr(self._fp, 'flush'):
             self._fp.flush()
         return ds
+
+
+# ---------------------------------------------------------------------------
+# statistics files
+# ---------------------------------------------------------------------------
+def _strand_byte(strand):
+    """the byte the most-significant table's S1 column stores for a strand"""
+    b = strand if isinstance(strand, bytes) else str(strand).encode()
+    return b[:1] if b else b'\0'
+
+
+class _StatsWriter(object):
+    _level = False
+    _dtype = MODEL_STATS_DTYPE
+
+    def __init__(self, h5_file, stat_type, region_size, cov_thresh, num_most_signif, ctx=None,
+                 device=0):
+        self._fp = h5_file
+        self.region_size = region_size
+        h5_file.attrs['stat_type'] = stat_type
+        h5_file.attrs['block_size'] = region_size
+        self.stat_blocks = h5_file.create_group(PER_READ_BLOCKS_NAME)
+        h5_file.attrs[COV_THRESH_NAME] = cov_thresh
+        self._init_extra()
+        self.most_signif_sites = h5_file.create_group(MOST_SIGNIF_NAME)
+        self.chrm_names = OrderedDict()
+        self.chrm_id_grp = self.most_signif_sites.create_group('chrm_ids')
+        self.curr_block_num = 0
+        self.is_empty = True
+        # the device table lives on the context, one per context: a writer owns a context
+        # unless given one, so writers open at once never share a table
+        self._own_ctx = ctx is None
+        self.ctx = _lib.Context(device) if ctx is None else ctx
+        self.ctx.most_signif_begin(self._level, num_most_signif)
+
+    def _init_extra(self):
+        pass
+
+    def _chrm_id(self, chrm):
+        if chrm not in self.chrm_names:
+            self.chrm_names[chrm] = len(self.chrm_names)
+        return self.chrm_names[chrm]
+
+    def write_block_table(self, table, chrm, strand, start):
+        """one ``Block_<n>`` group: its chrm / strand / start attributes and the table"""
+        grp = self.stat_blocks.create_group('Block_' + str(self.curr_block_num))
+        self.curr_block_num += 1
+        grp.attrs['chrm'] = chrm
+        grp.attrs['strand'] = strand
+        grp.attrs['start'] = start
+        grp.create_dataset('block_stats', data=table, compression='gzip')
+        self.is_empty = False
+
+    def _write_rows(self, table, chrm, strand, start):
+        self.write_block_table(table, chrm, strand, start)
+        cid = self._chrm_id(chrm)
+        key = table[self._dtype[0][0]]
+        self.ctx.most_signif_add_rows(
+            key, table['pos'], table['cov'], table['control_cov'], cid, _strand_byte(strand),
+            frac=None if self._level else table['frac'],
+            valid_cov=None if self._level else table['valid_cov'])
+
+    def most_signif_table(self):
+        """the most-significant table as ``_close_write`` stores it (trimmed when fewer rows
+        than requested exist)"""
+        c = self.ctx.most_signif_get()
+        out = np.empty(c['key'].shape[0], dtype=self._dtype + MOST_SIGNIF_EXTRA)
+        out[self._dtype[0][0]] = c['key']
+        for name, _ in self._dtype[1:] + MOST_SIGNIF_EXTRA:
+            out[name] = c[name]
+        return out
+
+    def close(self):
+        """``_close_write``: the most-significant dataset and the chromosome ids"""
+        self.most_signif_sites.create_dataset(MOST_SIGNIF_NAME, data=self.most_signif_table(),
+                                              compression='gzip')
+        for chrm_name, chrm_id in self.chrm_names.items():
+            self.chrm_id_grp.attrs[chrm_name] = chrm_id
+        self.discard()
+
+    def discard(self):
+        """close the device table (and the writer's own context) without writing it"""
+        self.ctx.most_signif_end()
+        if self._own_ctx:
+            self.ctx.close()
+
+
+class ModelStatsWriter(_StatsWriter):
+    """``ModelStats`` opened for writing (tombo_stats.py:2594-2636, 2737-2795) over an
+    h5py-like file: the reference's layout, with the running most-significant table on the
+    device.  ``cov_damp_counts`` is (unmod, mod).  Without ``ctx`` the writer opens a context
+    of its own on ``device`` (the table belongs to the context) and closes it in close()."""
+
+    def __init__(self, h5_file, stat_type, region_size, cov_damp_counts, cov_thresh,
+                 num_most_signif, ctx=None, device=0):
+        self.cov_damp_counts = dict(zip(('unmod', 'mod'), cov_damp_counts))
+        super(ModelStatsWriter, self).__init__(h5_file, stat_type, region_size, cov_thresh,
+                                               num_most_signif, ctx, device)
+
+    def _init_extra(self):
+        grp = self._fp.create_group(COV_DAMP_COUNTS_NAME)
+        grp.attrs['unmod'] = self.cov_damp_counts['unmod']
+        grp.attrs['mod'] = self.cov_damp_counts['mod']
+
+    def _write_stat_block(self, reg_stats):
+        """one ``regionStats`` (:2737-2773): the block table without NaN damp_frac rows; the
+        fields are zipped, so the shortest one sets the row count"""
+        fracs = np.asarray(reg_stats.reg_frac_standard_base, dtype=np.float64)
+        valid_cov = np.asarray(reg_stats.valid_cov)
+        damp = (np.round(fracs * valid_cov) + self.cov_damp_counts['unmod']) / (
+            valid_cov + sum(list(self.cov_damp_counts.values())))
+        cols = (damp, fracs, reg_stats.reg_poss, reg_stats.reg_cov, reg_stats.ctrl_cov, valid_cov)
+        n = min(len(c) for c in cols)
+        keep = ~np.isnan(damp[:n])
+        table = np.empty(int(keep.sum()), dtype=MODEL_STATS_DTYPE)
+        for (name, _), c in zip(MODEL_STATS_DTYPE, cols):
+            table[name] = np.asarray(c)[:n][keep]
+        self._write_rows(table, reg_stats.chrm, reg_stats.strand, reg_stats.start)
+
+    def write_aggregated(self, blocks, row_off, cols):
+        """the block tables of one tb2_stats_file_aggregate call: ``blocks`` (chrm, strand,
+        start) in order, ``cols`` its downloaded (pos, damp_frac, frac, cov, valid_cov); the
+        rows join the most-significant table without leaving the device"""
+        pos, damp, frac, cov, valid = cols
+        for b, (chrm, strand, start) in enumerate(blocks):
+            lo, hi = row_off[b], row_off[b + 1]
+            table = np.zeros(hi - lo, dtype=MODEL_STATS_DTYPE)
+            table['damp_frac'], table['frac'], table['pos'] = damp[lo:hi], frac[lo:hi], pos[lo:hi]
+            table['cov'], table['valid_cov'] = cov[lo:hi], valid[lo:hi]
+            self.write_block_table(table, chrm, strand, start)
+        self.ctx.most_signif_add_aggregate()
+
+
+class LevelStatsWriter(_StatsWriter):
+    """``LevelStats`` opened for writing (tombo_stats.py:3064-3099, 3194-3224)"""
+    _level = True
+    _dtype = LEVEL_STATS_DTYPE
+
+    def _write_stat_block(self, grp_stats):
+        """one ``groupStats``: the block table without NaN stat rows (zip semantics)"""
+        cols = (grp_stats.reg_stats, grp_stats.reg_poss, grp_stats.reg_cov, grp_stats.ctrl_cov)
+        n = min(len(c) for c in cols)
+        stat = np.asarray(grp_stats.reg_stats, dtype=np.float64)[:n]
+        keep = ~np.isnan(stat)
+        table = np.empty(int(keep.sum()), dtype=LEVEL_STATS_DTYPE)
+        for (name, _), c in zip(LEVEL_STATS_DTYPE, cols):
+            table[name] = np.asarray(c)[:n][keep]
+        self._write_rows(table, grp_stats.chrm, grp_stats.strand, grp_stats.start)

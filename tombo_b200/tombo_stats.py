@@ -27,7 +27,7 @@ __all__ = [
     'get_read_seg_score', 'calc_kmer_fitted_shift_scale', 'load_resquiggle_parameters',
     'compute_num_events', 'get_dynamic_prog_params', 'identify_stalls',
     'compute_alt_model_read_stats', 'compute_alt_model_reads_stats', 'trim_seq_and_means', 'apply_per_read_thresh',
-    'collate_reg_stats', 'calc_damp_fraction', 'calc_window_fishers_method',
+    'collate_reg_stats', 'calc_damp_fraction', 'aggregate_per_read_stats', 'calc_window_fishers_method',
     'compute_de_novo_read_stats', 'compute_sample_compare_read_stats',
     'compute_ks_tests', 'compute_u_tests', 'compute_t_tests', 'calc_window_means',
     'compute_group_reg_stats', 'get_reads_ref', 'compute_posterior_samp_dists',
@@ -586,6 +586,62 @@ def calc_damp_fraction(cov_damp_counts, fracs, valid_cov):
     non_mod_counts = np.round(fracs * valid_cov)
     return (non_mod_counts + cov_damp_counts['unmod']) / (
         valid_cov + sum(list(cov_damp_counts.values())))
+
+
+# per-read entries per tb2_stats_file_aggregate call (12 bytes each on the device)
+AGG_BATCH_ENTRIES = 1 << 24
+
+
+def aggregate_per_read_stats(pr_stats, single_read_thresh, lower_thresh, stats_file,
+                             cov_damp_counts, min_test_reads, num_most_signif, device=0,
+                             batch_entries=AGG_BATCH_ENTRIES, ctx=None):
+    """``tombo detect_modifications aggregate_per_read_stats`` (tombo_stats.py:4699-4777) with
+    one aggregation process: re-threshold a per-read statistics file into a statistics file.
+
+    ``pr_stats`` iterates as (chrm, strand, start, end, block_stats) and has ``stat_type`` and
+    ``region_size`` (the reference's ``PerReadStats``); ``stats_file`` is an h5py-like file
+    that receives the ``ModelStats`` layout (formats.ModelStatsWriter).  Blocks go to the
+    device in iteration order, which is the reference's arrival order, batched up to
+    ``batch_entries`` statistics per call.  ``min_test_reads`` is stored as the file's
+    coverage threshold; the reference filters nothing by it here.  ``ctx`` overrides the
+    device's default context."""
+    stat_type, region_size = pr_stats.stat_type, int(pr_stats.region_size)
+    writer = formats.ModelStatsWriter(stats_file, stat_type, region_size, cov_damp_counts,
+                                      min_test_reads, num_most_signif, ctx=ctx, device=device)
+    ctx, code = writer.ctx, 0 if stat_type == ALT_MODEL_TXT else 1
+    batch, n_entries = [], 0
+
+    def flush():
+        rows = np.zeros((len(batch), 5), dtype=np.int64)
+        off = 0
+        for b, (chrm, strand, start, bs) in enumerate(batch):
+            rows[b] = (start, off, bs.shape[0], writer._chrm_id(chrm),
+                       formats._strand_byte(strand)[0])
+            off += bs.shape[0]
+        pos = np.concatenate([bs['pos'] for _, _, _, bs in batch])
+        stat = np.concatenate([bs['stat'] for _, _, _, bs in batch])
+        row_off = ctx.stats_file_aggregate(
+            rows, region_size, pos, stat, single_read_thresh, lower_thresh, code,
+            writer.cov_damp_counts['unmod'], writer.cov_damp_counts['mod'])
+        writer.write_aggregated([b[:3] for b in batch], row_off,
+                                ctx.stats_file_download(int(row_off[-1])))
+        del batch[:]
+
+    try:
+        for chrm, strand, start, _, block_stats in pr_stats:
+            batch.append((chrm, strand, start, block_stats))
+            n_entries += block_stats.shape[0]
+            if n_entries >= batch_entries:
+                flush()
+                n_entries = 0
+        if batch:
+            flush()
+    except Exception:
+        writer.discard()
+        raise
+    writer.close()
+    if writer.is_empty:
+        raise th.TomboError('No genomic positions contain --minimum-test-reads.')
 
 
 # ---------------------------------------------------------------------------
