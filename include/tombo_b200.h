@@ -115,6 +115,9 @@ int tb2_device_count(void);
 int tb2_ctx_create(int device, tb2_ctx **out);
 void tb2_ctx_destroy(tb2_ctx *ctx);
 const char *tb2_status_message(int status);
+/* the message of the last call on this ctx, empty if that call set none: every call that
+ * takes a ctx starts from an empty message, except tb2_last_error, tb2_launch_count and
+ * tb2_last_timing, which report on the call before them */
 const char *tb2_last_error(tb2_ctx *ctx);
 /* kernels launched by this ctx since creation (bench.py "gpu_launches") */
 int64_t tb2_launch_count(tb2_ctx *ctx);
@@ -287,7 +290,9 @@ int tb2_pipeline_chunks(int sm_count, int64_t n_reads, int64_t *starts_out, int 
 /* The same call in three stages, for callers that keep inputs resident in HBM or
  * overlap transfers themselves: upload (H2D of raw / seq, allocation), compute
  * (kernels only, results stay on the device), download (D2H into caller buffers
- * laid out as in tb2_resquiggle_batch).  compute may be repeated on one upload. */
+ * laid out as in tb2_resquiggle_batch).  compute may be repeated on one upload.  A failed
+ * upload leaves no batch, a failed compute no results: the calls that need them return
+ * TB2_ERR_INVALID_ARG until the next successful upload / compute. */
 int tb2_batch_upload(tb2_ctx *ctx, int64_t n_reads, const void *raw, int raw_dtype,
                      const int64_t *raw_off, const uint8_t *seq,
                      const int64_t *seq_off, const tb2_params *params,
@@ -351,7 +356,9 @@ int tb2_timer_stop(tb2_ctx *ctx, double *ms_out);
  * positions stay on the device for tb2_region_stats_add_batch_llr; tb2_batch_llr_download
  * copies them out (site_off has n_reads + 1 entries; llr_out / pos_out sized
  * *n_sites_total).  Single-base motif, whole '+' strand reads; any motif, both strands and
- * a region: tb2_batch_alt_llr_motif. */
+ * a region: tb2_batch_alt_llr_motif.  A failed call of either leaves no LLRs resident:
+ * tb2_batch_llr_download and tb2_region_stats_add_batch_llr then return
+ * TB2_ERR_INVALID_ARG until the next successful one. */
 int tb2_batch_alt_llr(tb2_ctx *ctx, const int64_t *read_start, int alt_base_code,
                       int use_standard_llhr, double scale_factor, double height_factor,
                       double height_power, int64_t *n_sites_total);
@@ -460,7 +467,9 @@ int tb2_de_novo_read_stats_batch(tb2_ctx *ctx, int64_t n_reads, const double *no
  * filled); pvals_out / pos_out hold up to sum(nb) entries.  read_status (nullable, n_reads)
  * gets 0 or the code of the TomboError the reference raises for the read; such a read has no
  * statistics.  The statistics also stay on the device for tb2_region_stats_add_tests, until
- * the next call of either function or of tb2_batch_de_novo_region.  fm_offset 0 .. 64.
+ * the next call of either function or of tb2_batch_de_novo_region; a failed call of any of
+ * the three leaves none, and tb2_region_stats_add_tests returns TB2_ERR_INVALID_ARG until
+ * the next successful one.  fm_offset 0 .. 64.
  * tb2_last_timing out[0] is the kernel time.
  *
  * tb2_de_novo_region_stats: compute_de_novo_read_stats (:3771-3873) with the canonical model
@@ -678,10 +687,11 @@ typedef struct tb2_sf_block {
  * covered positions in ascending order without those whose damp_frac is NaN; row_off
  * (n_blocks + 1, caller's) receives their offsets.  control_cov is 0 for every row (:2756).
  * The rows stay on the device for tb2_stats_file_aggregate_download and
- * tb2_most_signif_add_aggregate until the next call.  A position outside [start, start +
- * region_size), an invalid block range, region_size outside 1 .. 2^28 or a NaN threshold or
- * pseudo-count -> TB2_ERR_INVALID_ARG; a buffer that does not fit on the device ->
- * TB2_ERR_CAPACITY.  tb2_last_timing out[0] is the kernel time. */
+ * tb2_most_signif_add_aggregate until the next call; a failed call leaves none, and those
+ * two return TB2_ERR_INVALID_ARG until the next successful one.  A position outside
+ * [start, start + region_size), an invalid block range, region_size outside 1 .. 2^28 or a
+ * NaN threshold or pseudo-count -> TB2_ERR_INVALID_ARG; a buffer that does not fit on the
+ * device -> TB2_ERR_CAPACITY.  tb2_last_timing out[0] is the kernel time. */
 int tb2_stats_file_aggregate(tb2_ctx *ctx, int64_t n_blocks, const int64_t *blocks,
                              int64_t region_size, int64_t n_stat, const uint32_t *pos,
                              const double *stat, double single_read_thresh, double lower_thresh,

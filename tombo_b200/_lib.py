@@ -319,8 +319,9 @@ class Context(object):
     def check(self, rc):
         if rc != 0:
             msg = status_message(rc)
-            if rc == 200:
-                msg += ': ' + self.lib.tb2_last_error(self.handle).decode()
+            err = self.lib.tb2_last_error(self.handle).decode()
+            if err:
+                msg += ': ' + err
             raise TomboB200Error('tombo_b200 call failed (%d): %s' % (rc, msg))
 
     def launch_count(self):
@@ -1031,15 +1032,11 @@ class Context(object):
         if pos.shape != stat.shape:
             raise ValueError('pos and stat need the same length')
         row_off = np.zeros(blocks.shape[0] + 1, dtype=np.int64)
-        rc = self.lib.tb2_stats_file_aggregate(
+        self.check(self.lib.tb2_stats_file_aggregate(
             self.handle, blocks.shape[0], ptr(blocks, i64), int(region_size), stat.shape[0],
             ptr(pos, C.c_uint32), ptr(stat, f64), float(single_read_thresh),
             float('nan') if lower_thresh is None else float(lower_thresh), int(stat_type),
-            float(unmod_count), float(mod_count), ptr(row_off, i64))
-        err = self.lib.tb2_last_error(self.handle).decode() if rc == TB2_ERR_INVALID_ARG else ''
-        if err:
-            raise TomboB200Error('tb2_stats_file_aggregate: ' + err)
-        self.check(rc)
+            float(unmod_count), float(mod_count), ptr(row_off, i64)))
         return row_off
 
     def stats_file_download(self, n_rows):
@@ -1053,10 +1050,7 @@ class Context(object):
 
     def most_signif_begin(self, level, num_most_signif):
         """open this context's table; raises while another is open"""
-        rc = self.lib.tb2_most_signif_begin(self.handle, int(bool(level)), int(num_most_signif))
-        if rc == TB2_ERR_INVALID_ARG and self.lib.tb2_last_error(self.handle):
-            raise TomboB200Error('tb2_most_signif_begin: ' + self.lib.tb2_last_error(self.handle).decode())
-        self.check(rc)
+        self.check(self.lib.tb2_most_signif_begin(self.handle, int(bool(level)), int(num_most_signif)))
 
     def most_signif_end(self):
         self.check(self.lib.tb2_most_signif_end(self.handle))

@@ -361,26 +361,14 @@ k_acc_rates(const unsigned char *lab, const unsigned long long *texcl, long long
 // ---------------------------------------------------------------------------
 // host side
 // ---------------------------------------------------------------------------
-#define ACC_RESERVE(ctx, buf, bytes)                                                    \
-    do {                                                                                \
-        if ((buf).reserve(bytes) != cudaSuccess) {                                      \
-            cudaGetLastError();                                                         \
-            char _b[160];                                                               \
-            snprintf(_b, sizeof(_b), "accuracy: cannot allocate %zu bytes on the device", \
-                     (size_t)(bytes));                                                  \
-            (ctx)->err = _b;                                                            \
-            return TB2_ERR_CAPACITY;                                                    \
-        }                                                                               \
-    } while (0)
-
 // grow a slot to hold `need` entries, keeping its first s.n
 int slot_reserve(tb2_ctx *ctx, Slot &s, long long need)
 {
     if ((size_t)need * 8 + 8 <= s.stat.cap && (size_t)need + 8 <= s.lab.cap) return TB2_OK;
     DevBuf st, lb;
     const size_t want = (size_t)need + (size_t)need / 2;
-    ACC_RESERVE(ctx, st, want * 8 + 8);
-    ACC_RESERVE(ctx, lb, want + 8);
+    TB2_RESERVE(ctx, "accuracy", st, want * 8 + 8);
+    TB2_RESERVE(ctx, "accuracy", lb, want + 8);
     if (s.n) {
         TB2_CUDA_TRY(ctx, cudaMemcpyAsync(st.p, s.stat.p, (size_t)s.n * 8, cudaMemcpyDeviceToDevice, ctx->stream));
         TB2_CUDA_TRY(ctx, cudaMemcpyAsync(lb.p, s.lab.p, (size_t)s.n, cudaMemcpyDeviceToDevice, ctx->stream));
@@ -393,7 +381,7 @@ int slot_reserve(tb2_ctx *ctx, Slot &s, long long need)
 
 template <class T> int acc_upload(tb2_ctx *ctx, DevBuf &b, const T *host, long long n)
 {
-    ACC_RESERVE(ctx, b, (size_t)n * sizeof(T) + 8);
+    TB2_RESERVE(ctx, "accuracy", b, (size_t)n * sizeof(T) + 8);
     if (n) TB2_CUDA_TRY(ctx, cudaMemcpyAsync(b.p, host, (size_t)n * sizeof(T), cudaMemcpyHostToDevice, ctx->stream));
     return TB2_OK;
 }
@@ -458,12 +446,12 @@ int label(tb2_ctx *ctx, AccArgs &a, long long n_blocks, const int32_t *slot_of, 
     cudaStream_t q = ctx->stream;
     const int nm = MODE == MODE_TRUTH ? 1 : a.n_motifs;
     std::vector<long long> cnt((size_t)n_blocks * nm);
-    ACC_RESERVE(ctx, P[A_CNT], cnt.size() * 8 + 16);
+    TB2_RESERVE(ctx, "accuracy", P[A_CNT], cnt.size() * 8 + 16);
     int *fail = (int *)(P[A_CNT].as<long long>() + cnt.size());
     TB2_CUDA_TRY(ctx, cudaEventRecord(ctx->ev0, q));          // kernel time: tb2_last_timing
     TB2_CUDA_TRY(ctx, cudaMemsetAsync(fail, 0, 4, q));
     if (MODE == MODE_CTRL && n_blocks && a.n_seq) {
-        ACC_RESERVE(ctx, P[A_SITE], (size_t)nm * a.n_seq);
+        TB2_RESERVE(ctx, "accuracy", P[A_SITE], (size_t)nm * a.n_seq);
         TB2_CUDA_TRY(ctx, cudaMemsetAsync(P[A_SITE].p, 0, (size_t)nm * a.n_seq, q));
         a.site = P[A_SITE].as<unsigned char>();
         k_acc_sites<<<dim3((unsigned)n_blocks, (unsigned)nm), AT, 0, q>>>(a, P[A_SITE].as<unsigned char>());
@@ -553,9 +541,9 @@ int rates(tb2_ctx *ctx, const unsigned char *lab, long long n, long long n_point
     cudaStream_t q = ctx->stream;
     const long long n_tiles = (n + TILE - 1) / TILE;
     int rc;
-    ACC_RESERVE(ctx, P[A_GHIST], (size_t)(n_tiles + 1) * 8);
-    ACC_RESERVE(ctx, P[A_IDX], (size_t)2 * n_points * 8 + 8);
-    ACC_RESERVE(ctx, P[A_OUT], (size_t)3 * n_points * 8 + 8);
+    TB2_RESERVE(ctx, "accuracy", P[A_GHIST], (size_t)(n_tiles + 1) * 8);
+    TB2_RESERVE(ctx, "accuracy", P[A_IDX], (size_t)2 * n_points * 8 + 8);
+    TB2_RESERVE(ctx, "accuracy", P[A_OUT], (size_t)3 * n_points * 8 + 8);
     unsigned long long *tsum = P[A_GHIST].as<unsigned long long>();
     long long *idx = P[A_IDX].as<long long>();
     double *out = P[A_OUT].as<double>();
@@ -731,7 +719,6 @@ extern "C" int tb2_accuracy_curve(tb2_ctx *ctx, int slot, int64_t n_points, cons
 {
     int rc = tb2_use(ctx);
     if (rc) return rc;
-    ctx->err.clear();
     if (slot < 0 || slot >= MAXSLOT) return TB2_ERR_INVALID_ARG;
     AccuracyState &S = tb2_state(ctx->accuracy);
     Slot &s = S.slot[slot];
@@ -741,13 +728,13 @@ extern "C" int tb2_accuracy_curve(tb2_ctx *ctx, int slot, int64_t n_points, cons
     DevBuf *P = S.buf;
     cudaStream_t q = ctx->stream;
     const long long n_tiles = (n + TILE - 1) / TILE;
-    ACC_RESERVE(ctx, P[A_KEY0], (size_t)n * 8);
-    ACC_RESERVE(ctx, P[A_KEY1], (size_t)n * 8);
-    ACC_RESERVE(ctx, P[A_LAB0], (size_t)n);
-    ACC_RESERVE(ctx, P[A_LAB1], (size_t)n);
-    ACC_RESERVE(ctx, P[A_THIST], (size_t)256 * n_tiles * 4);
-    ACC_RESERVE(ctx, P[A_TOFF], (size_t)256 * n_tiles * 8);
-    ACC_RESERVE(ctx, P[A_CNT], (size_t)9 * 256 * 8 + 8);
+    TB2_RESERVE(ctx, "accuracy", P[A_KEY0], (size_t)n * 8);
+    TB2_RESERVE(ctx, "accuracy", P[A_KEY1], (size_t)n * 8);
+    TB2_RESERVE(ctx, "accuracy", P[A_LAB0], (size_t)n);
+    TB2_RESERVE(ctx, "accuracy", P[A_LAB1], (size_t)n);
+    TB2_RESERVE(ctx, "accuracy", P[A_THIST], (size_t)256 * n_tiles * 4);
+    TB2_RESERVE(ctx, "accuracy", P[A_TOFF], (size_t)256 * n_tiles * 8);
+    TB2_RESERVE(ctx, "accuracy", P[A_CNT], (size_t)9 * 256 * 8 + 8);
     unsigned long long *gh = P[A_CNT].as<unsigned long long>();
     int *nan_flag = (int *)(gh + 9 * 256);
     TB2_CUDA_TRY(ctx, cudaEventRecord(ctx->ev0, q));          // kernel time: tb2_last_timing

@@ -116,6 +116,20 @@ struct tb2_ctx {
         TB2_CUDA_TRY(ctx, cudaGetLastError());                                         \
     } while (0)
 
+// grow a DevBuf; a device that cannot hold it is TB2_ERR_CAPACITY, with `what` (the module)
+// and the size in the message
+#define TB2_RESERVE(ctx, what, buf, bytes)                                             \
+    do {                                                                               \
+        if ((buf).reserve(bytes) != cudaSuccess) {                                     \
+            cudaGetLastError();                                                        \
+            char _b[160];                                                              \
+            snprintf(_b, sizeof(_b), "%s: cannot allocate %zu bytes on the device",    \
+                     what, (size_t)(bytes));                                           \
+            (ctx)->err = _b;                                                           \
+            return TB2_ERR_CAPACITY;                                                   \
+        }                                                                              \
+    } while (0)
+
 // a module's state on the context, created on first use.  Called where T is complete: the
 // shared_ptr keeps T's deleter, so tb2_ctx_destroy frees it without knowing the type.
 template <class T> T &tb2_state(std::shared_ptr<T> &state)
@@ -140,9 +154,12 @@ static inline int tb2_record_kernel_time(tb2_ctx *ctx, cudaEvent_t split_at = nu
     return TB2_OK;
 }
 
+// the first statement of every entry point that takes a context: tb2_last_error then holds
+// the message of this call only (empty if it sets none)
 static inline int tb2_use(tb2_ctx *ctx)
 {
     if (!ctx) return TB2_ERR_INVALID_ARG;
+    ctx->err.clear();
     cudaError_t e = cudaSetDevice(ctx->device);
     if (e != cudaSuccess) { ctx->err = cudaGetErrorString(e); return TB2_ERR_CUDA; }
     return TB2_OK;

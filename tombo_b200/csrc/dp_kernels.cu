@@ -423,7 +423,8 @@ static int run_single(tb2_ctx *ctx, int mode, const double *em, int64_t n_em, co
 {
     int rc = tb2_use(ctx);
     if (rc) return rc;
-    if (!em || !rm || !rs || !p || n_em < 1 || nb < 1) return TB2_ERR_INVALID_ARG;
+    if (!em || !rm || !rs || !p || n_em < 1 || nb < 1 || (mode == 0 ? !tb_out : (!start_loc || !epb)))
+        return TB2_ERR_INVALID_ARG;
     auto &P = tb2_state(ctx->dp).buf;
     cudaStream_t s = ctx->stream;
     const long long W = mode == 0 ? std::max<long long>(1, n_em - std::min<long long>(nb, n_em) / 4)
@@ -470,7 +471,6 @@ extern "C" int tb2_find_static_base_assignment(tb2_ctx *ctx, const double *event
                                                const tb2_params *params, int64_t *read_tb_out,
                                                int *read_status)
 {
-    if (!read_tb_out) return TB2_ERR_INVALID_ARG;
     return run_single(ctx, 0, event_means, n_events, ref_means, ref_sds, n_bases, params, 0, 0, 0,
                       0.0, read_tb_out, n_bases + 1, nullptr, nullptr, read_status);
 }
@@ -483,7 +483,6 @@ extern "C" int tb2_find_seq_start_in_events(tb2_ctx *ctx, const double *event_me
                                             double sig_match_thresh, int64_t *start_loc,
                                             double *events_per_base, int *read_status)
 {
-    if (!start_loc || !events_per_base || num_bases < 1 || num_events < 1) return TB2_ERR_INVALID_ARG;
     return run_single(ctx, 1, event_means, n_events, ref_means, ref_sds, n_ref, params, num_bases,
                       num_events, check_score, sig_match_thresh, nullptr, 0, start_loc,
                       events_per_base, read_status);

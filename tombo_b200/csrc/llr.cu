@@ -17,8 +17,8 @@ enum { L_MEAN = 0, L_MOFF, L_SEQ, L_SOFF, L_START, L_CNT, L_SITEOFF, L_LLR, L_PO
 
 struct LlrState {
     DevBuf scratch[L_COUNT];
-    // resident LLRs of the last tb2_batch_alt_llr, for tb2_batch_llr_download and
-    // tb2_region_stats_add_batch_llr
+    // resident LLRs of the last successful tb2_batch_alt_llr[_motif], for
+    // tb2_batch_llr_download and tb2_region_stats_add_batch_llr; reads == 0: none
     DevBuf site_off, llr, pos;
     long long sites = 0;
     int reads = 0;
@@ -174,7 +174,8 @@ int run_host(tb2_ctx *ctx, LlrKernel<A> count, LlrKernel<A> fill, const A &a, in
 }
 
 // resident calls: the LLRs stay in LlrState for tb2_batch_llr_download and
-// tb2_region_stats_add_batch_llr
+// tb2_region_stats_add_batch_llr.  The caller dropped the previous ones on entry; these
+// are published only once complete.
 template <class A>
 int run_resident(tb2_ctx *ctx, LlrKernel<A> count, LlrKernel<A> fill, const A &a,
                  const BatchResultView &v, int32_t *read_status, int64_t *n_sites_total)
@@ -223,6 +224,8 @@ extern "C" int tb2_batch_alt_llr(tb2_ctx *ctx, const int64_t *read_start, int al
 {
     int rc = tb2_use(ctx);
     if (rc) return rc;
+    LlrState &L = tb2_state(ctx->llr);
+    L.reads = 0; L.sites = 0;
     if (!read_start || alt_base_code < 0 || alt_base_code > 3 || !alt_model_ok(ctx))
         return TB2_ERR_INVALID_ARG;
     LlrArgs a = llr_args(ctx, alt_base_code, use_standard_llhr, scale_factor, height_factor, height_power);
@@ -309,6 +312,8 @@ extern "C" int tb2_batch_alt_llr_motif(tb2_ctx *ctx, const int64_t *read_start, 
 {
     int rc = tb2_use(ctx);
     if (rc) return rc;
+    LlrState &L = tb2_state(ctx->llr);
+    L.reads = 0; L.sites = 0;
     if (!read_start || !strand) return TB2_ERR_INVALID_ARG;
     MotifArgs a;
     if ((rc = motif_args(ctx, motif, max_motif_bb, max_motif_ab, reg_start, reg_end,
@@ -325,7 +330,10 @@ extern "C" int tb2_batch_llr_download(tb2_ctx *ctx, double *llr_out, int64_t *po
     int rc = tb2_use(ctx);
     if (rc) return rc;
     const LlrState &L = tb2_state(ctx->llr);
-    if (L.reads <= 0 || !site_off) return TB2_ERR_INVALID_ARG;
+    if (L.reads <= 0 || !site_off) {
+        ctx->err = "no successful tb2_batch_alt_llr / tb2_batch_alt_llr_motif call, or a NULL site_off";
+        return TB2_ERR_INVALID_ARG;
+    }
     cudaStream_t s = ctx->stream;
     const size_t t = (size_t)L.sites;
     if (t && (!llr_out || !pos_out)) return TB2_ERR_INVALID_ARG;
@@ -345,7 +353,10 @@ extern "C" int tb2_region_stats_add_batch_llr(tb2_ctx *ctx, double single_read_t
     int rc = tb2_use(ctx);
     if (rc) return rc;
     LlrState &L = tb2_state(ctx->llr);
-    if (L.reads <= 0 || isnan(single_read_thresh)) return TB2_ERR_INVALID_ARG;
+    if (L.reads <= 0 || isnan(single_read_thresh)) {
+        ctx->err = "no successful tb2_batch_alt_llr / tb2_batch_alt_llr_motif call, or a NaN threshold";
+        return TB2_ERR_INVALID_ARG;
+    }
     return tb2_region_accumulate_dev(ctx, L.sites, L.llr.as<double>(), L.pos.as<long long>(),
                                      single_read_thresh, lower_thresh, stat_type);
 }

@@ -368,12 +368,12 @@ static int batch_upload_impl(tb2_ctx *ctx, int64_t n_reads, const void *raw, int
 {
     int rc = tb2_use(ctx);
     if (rc) return rc;
+    BatchHolder *h = holder_of(ctx);
+    h->uploaded = h->computed = false;
     if (n_reads < 1 || n_reads > 0x7ffffff0 || !raw || !seq || !raw_off || !seq_off || !params ||
         !policy || (raw_dtype != 0 && raw_dtype != 1))
         return TB2_ERR_INVALID_ARG;
     if (ctx->kmer_width <= 0) { ctx->err = "tb2_set_model has not been called"; return TB2_ERR_INVALID_ARG; }
-    BatchHolder *h = holder_of(ctx);
-    h->uploaded = h->computed = false;
     const int n = (int)n_reads;
     rc = build_view(ctx, h->buf, n, raw_off, seq_off, ctx->kmer_width, *params,
                     policy->min_event_to_seq_ratio, (int)policy->is_rna, h->hb, h->v);
@@ -460,11 +460,11 @@ static int batch_compute_impl(tb2_ctx *ctx, const tb2_params *params,
 {
     int rc = tb2_use(ctx);
     if (rc) return rc;
+    BatchHolder *h = holder_of(ctx);
+    h->computed = false;
     if (!params || !policy) return TB2_ERR_INVALID_ARG;
     if (policy->rescue && !save_params) return TB2_ERR_INVALID_ARG;
-    BatchHolder *h = holder_of(ctx);
     if (!h->uploaded) { ctx->err = "tb2_batch_upload has not been called"; return TB2_ERR_INVALID_ARG; }
-    h->computed = false;
     StagePolicy sp = stage_policy(*policy);
     sp.read_index_base = ctx->read_index_base;
     const HostBatch &hb = h->hb;
@@ -706,6 +706,7 @@ static int resquiggle_batch_impl(tb2_ctx *ctx, int64_t n_reads, const void *raw,
         ln->model_means.owned = ln->model_sds.owned = false;
         ln->kmer_width = ctx->kmer_width; ln->central_pos = ctx->central_pos;
         ln->async_mode = true;
+        ln->err.clear();      // no lane may report a message of an earlier call below
     }
     const int K = ctx->kmer_width;
     const int n = (int)n_reads;

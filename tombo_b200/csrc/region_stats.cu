@@ -43,8 +43,9 @@ struct RegionState {
     bool open = false;
     DevBuf cnt;
     DevBuf scratch[RS_COUNT];
-    // statistics and positions of the last de novo / sample-compare region call, for
-    // tb2_region_stats_add_tests; tests_n < 0: no such call yet
+    // statistics and positions of the last successful de novo / sample-compare region call,
+    // for tb2_region_stats_add_tests; tests_n < 0: none.  Each of those calls sets -1 on
+    // entry and its count only once it has succeeded.
     DevBuf tests_stat, tests_pos;
     long long tests_n = -1;
 };
@@ -545,10 +546,11 @@ extern "C" int tb2_de_novo_region_stats(tb2_ctx *ctx, int64_t n_reads, const dou
 {
     int rc = tb2_use(ctx);
     if (rc) return rc;
+    RegionState &R = tb2_state(ctx->region);
+    R.tests_n = -1;
     if (!stat_off) return TB2_ERR_INVALID_ARG;
     if ((rc = model_ok(ctx)) || (rc = region_args_ok(ctx, n_reads, strand, fm_offset, reg_start, reg_end)))
         return rc;
-    RegionState &R = tb2_state(ctx->region);
     DeNovoArgs a;
     memset(&a, 0, sizeof(a));
     if ((rc = tb2_stage_reads(ctx, n_reads, norm_mean, mean_off, seq, seq_off, read_start, R.scratch + F_MEAN, a.f)))
@@ -558,8 +560,7 @@ extern "C" int tb2_de_novo_region_stats(tb2_ctx *ctx, int64_t n_reads, const dou
     const long long total = de_novo_reads(ctx, n, (const long long *)mean_off, read_start, strand,
                                           fm_offset, reg_start, reg_end, rd, stat_off);
     if (total > 0 && (!pvals_out || !pos_out)) return TB2_ERR_INVALID_ARG;
-    R.tests_n = 0;
-    if (n == 0) return TB2_OK;
+    if (n == 0) { R.tests_n = 0; return TB2_OK; }
     de_novo_args(ctx, fm_offset, a);
     a.check = 1;
     if ((rc = run_de_novo(ctx, a, rd, total, R.tests_stat, R.tests_pos, pvals_out, pos_out, read_status)))
@@ -575,19 +576,19 @@ extern "C" int tb2_batch_de_novo_region(tb2_ctx *ctx, const int64_t *read_start,
 {
     int rc = tb2_use(ctx);
     if (rc) return rc;
+    RegionState &R = tb2_state(ctx->region);
+    R.tests_n = -1;
     if (!read_start || !strand) return TB2_ERR_INVALID_ARG;
     if ((rc = model_ok(ctx))) return rc;
     BatchResultView v;
     if ((rc = tb2_batch_result_view(ctx, &v))) return rc;
     if ((rc = region_args_ok(ctx, v.n_reads, strand, fm_offset, reg_start, reg_end))) return rc;
-    RegionState &R = tb2_state(ctx->region);
     const int n = v.n_reads;
     std::vector<DeNovoRead> rd;
     std::vector<int64_t> off(stat_off ? 0 : n + 1);
     const long long total = de_novo_reads(ctx, n, v.host_base_off, read_start, strand, fm_offset,
                                           reg_start, reg_end, rd, stat_off ? stat_off : off.data());
-    R.tests_n = 0;
-    if (n == 0) return TB2_OK;
+    if (n == 0) { R.tests_n = 0; return TB2_OK; }
     DeNovoArgs a;
     memset(&a, 0, sizeof(a));
     a.f.norm_mean = v.norm_mean; a.f.mean_off = v.base_off; a.f.seq = v.seq; a.f.seq_off = v.seq_off;
@@ -609,6 +610,8 @@ extern "C" int tb2_sample_compare_region_stats(tb2_ctx *ctx, int64_t n_reads, co
 {
     int rc = tb2_use(ctx);
     if (rc) return rc;
+    RegionState &R = tb2_state(ctx->region);
+    R.tests_n = -1;
     if (!stat_off || !ctrl_means || !ctrl_sds || !mean_off || (n_reads > 0 && !read_start))
         return TB2_ERR_INVALID_ARG;
     if ((rc = region_args_ok(ctx, n_reads, strand, fm_offset, reg_start, reg_end))) return rc;
@@ -619,7 +622,6 @@ extern "C" int tb2_sample_compare_region_stats(tb2_ctx *ctx, int64_t n_reads, co
         if (nb < 0 || nb > INT_MAX) return TB2_ERR_INVALID_ARG;
     }
     if (mean_off[n] > mean_off[0] && !norm_mean) return TB2_ERR_INVALID_ARG;
-    RegionState &R = tb2_state(ctx->region);
     auto &P = R.scratch;
     cudaStream_t s = ctx->stream;
     // host staging (:3713-3740): clip by fm_offset, flip '-' reads to genome order, and slice
@@ -666,9 +668,8 @@ extern "C" int tb2_sample_compare_region_stats(tb2_ctx *ctx, int64_t n_reads, co
     TB2_CUDA_TRY(ctx, P[F_LOGP].reserve((size_t)staged * 8 + 8));
     TB2_CUDA_TRY(ctx, R.tests_stat.reserve((size_t)staged * 8 + 8));
     TB2_CUDA_TRY(ctx, R.tests_pos.reserve((size_t)staged * 8 + 8));
-    R.tests_n = 0;
     stat_off[0] = 0;
-    if (n == 0) return TB2_OK;
+    if (n == 0) { R.tests_n = 0; return TB2_OK; }
     FisherArgs a;
     memset(&a, 0, sizeof(a));
     a.means = P[F_MEAN].as<double>(); a.rm = P[F_RM].as<double>(); a.rs = P[F_RS].as<double>();

@@ -62,18 +62,6 @@ namespace {
 // ---------------------------------------------------------------------------
 // host side
 // ---------------------------------------------------------------------------
-#define SF_RESERVE(ctx, buf, bytes)                                                     \
-    do {                                                                                \
-        if ((buf).reserve(bytes) != cudaSuccess) {                                      \
-            cudaGetLastError();                                                         \
-            char _b[160];                                                               \
-            snprintf(_b, sizeof(_b), "stats file: cannot allocate %zu bytes on the device", \
-                     (size_t)(bytes));                                                  \
-            (ctx)->err = _b;                                                            \
-            return TB2_ERR_CAPACITY;                                                    \
-        }                                                                               \
-    } while (0)
-
 unsigned grid_of(long long n) { return (unsigned)std::max<long long>(1, (n + 255) / 256); }
 
 // room for `need` rows, keeping the first S.n
@@ -86,7 +74,7 @@ int table_reserve(tb2_ctx *ctx, StatsFileState &S, long long need)
     }
     const long long cap = std::min<long long>((1LL << 32) - 1, std::max(need + need / 4, 2 * S.N));
     DevBuf nb;
-    SF_RESERVE(ctx, nb, (size_t)S.K * cap * 8);
+    TB2_RESERVE(ctx, "stats file", nb, (size_t)S.K * cap * 8);
     for (int w = 0; w < S.K && S.n; ++w)
         TB2_CUDA_TRY(ctx, cudaMemcpyAsync(nb.as<unsigned long long>() + (size_t)w * cap,
                                           S.tab[T_RAW].as<unsigned long long>() + (size_t)w * S.cap,
@@ -107,14 +95,14 @@ int table_reduce(tb2_ctx *ctx, StatsFileState &S)
     const long long n = S.n, m = std::min(S.n, S.N), cap = S.cap;
     const int K = S.K;
     const long long n_tiles = (n + RADIX_TILE - 1) / RADIX_TILE;
-    SF_RESERVE(ctx, T[T_OUT], (size_t)K * cap * 8);
-    SF_RESERVE(ctx, T[T_KEY0], (size_t)n * 8);
-    SF_RESERVE(ctx, T[T_KEY1], (size_t)n * 8);
-    SF_RESERVE(ctx, T[T_IDX0], (size_t)n * 4);
-    SF_RESERVE(ctx, T[T_IDX1], (size_t)n * 4);
-    SF_RESERVE(ctx, T[T_THIST], (size_t)256 * n_tiles * 4);
-    SF_RESERVE(ctx, T[T_TOFF], (size_t)256 * n_tiles * 8);
-    SF_RESERVE(ctx, T[T_HIST], (size_t)MAXW * 8 * 256 * 8);
+    TB2_RESERVE(ctx, "stats file", T[T_OUT], (size_t)K * cap * 8);
+    TB2_RESERVE(ctx, "stats file", T[T_KEY0], (size_t)n * 8);
+    TB2_RESERVE(ctx, "stats file", T[T_KEY1], (size_t)n * 8);
+    TB2_RESERVE(ctx, "stats file", T[T_IDX0], (size_t)n * 4);
+    TB2_RESERVE(ctx, "stats file", T[T_IDX1], (size_t)n * 4);
+    TB2_RESERVE(ctx, "stats file", T[T_THIST], (size_t)256 * n_tiles * 4);
+    TB2_RESERVE(ctx, "stats file", T[T_TOFF], (size_t)256 * n_tiles * 8);
+    TB2_RESERVE(ctx, "stats file", T[T_HIST], (size_t)MAXW * 8 * 256 * 8);
     unsigned long long *raw = T[T_RAW].as<unsigned long long>(), *gh = T[T_HIST].as<unsigned long long>();
     TB2_CUDA_TRY(ctx, cudaMemsetAsync(gh, 0, (size_t)K * 8 * 256 * 8, q));
     const unsigned hgrid = (unsigned)std::min<long long>(grid_of(n), 4LL * ctx->sm_count);
@@ -181,7 +169,6 @@ extern "C" int tb2_stats_file_aggregate(tb2_ctx *ctx, int64_t n_blocks, const in
 {
     int rc = tb2_use(ctx);
     if (rc) return rc;
-    ctx->err.clear();
     StatsFileState &S = tb2_state(ctx->stats_file);
     S.agg_blocks = -1;
     const tb2_sf_block *blk = (const tb2_sf_block *)block_rows;
@@ -202,18 +189,18 @@ extern "C" int tb2_stats_file_aggregate(tb2_ctx *ctx, int64_t n_blocks, const in
     DevBuf *G = S.agg;
     cudaStream_t q = ctx->stream;
     const long long U = ub[n_blocks];
-    SF_RESERVE(ctx, G[G_BLK], (size_t)n_blocks * sizeof(tb2_sf_block) + 8);
-    SF_RESERVE(ctx, G[G_POS], (size_t)n_stat * 4 + 8);
-    SF_RESERVE(ctx, G[G_STAT], (size_t)n_stat * 8 + 8);
-    SF_RESERVE(ctx, G[G_UB], (size_t)(n_blocks + 1) * 8);
-    SF_RESERVE(ctx, G[G_CNT], (size_t)n_blocks * 8 + 8);
-    SF_RESERVE(ctx, G[G_OFF], (size_t)(n_blocks + 1) * 8);
-    SF_RESERVE(ctx, G[G_ERR], 8);
+    TB2_RESERVE(ctx, "stats file", G[G_BLK], (size_t)n_blocks * sizeof(tb2_sf_block) + 8);
+    TB2_RESERVE(ctx, "stats file", G[G_POS], (size_t)n_stat * 4 + 8);
+    TB2_RESERVE(ctx, "stats file", G[G_STAT], (size_t)n_stat * 8 + 8);
+    TB2_RESERVE(ctx, "stats file", G[G_UB], (size_t)(n_blocks + 1) * 8);
+    TB2_RESERVE(ctx, "stats file", G[G_CNT], (size_t)n_blocks * 8 + 8);
+    TB2_RESERVE(ctx, "stats file", G[G_OFF], (size_t)(n_blocks + 1) * 8);
+    TB2_RESERVE(ctx, "stats file", G[G_ERR], 8);
     const int cols[5] = {G_UPOS, G_UDAMP, G_UFRAC, G_UCOV, G_UVALID}, pcols[5] = {G_POSO, G_DAMP, G_FRAC, G_COV, G_VALID};
     const int width[5] = {4, 8, 8, 4, 4};
     for (int c = 0; c < 5; ++c) {
-        SF_RESERVE(ctx, G[cols[c]], (size_t)U * width[c] + 8);
-        SF_RESERVE(ctx, G[pcols[c]], (size_t)U * width[c] + 8);
+        TB2_RESERVE(ctx, "stats file", G[cols[c]], (size_t)U * width[c] + 8);
+        TB2_RESERVE(ctx, "stats file", G[pcols[c]], (size_t)U * width[c] + 8);
     }
     if (n_blocks)
         TB2_CUDA_TRY(ctx, cudaMemcpyAsync(G[G_BLK].p, blk, (size_t)n_blocks * sizeof(tb2_sf_block),
@@ -248,7 +235,7 @@ extern "C" int tb2_stats_file_aggregate(tb2_ctx *ctx, int64_t n_blocks, const in
         TB2_CHECK_LAUNCH(ctx);
     } else if (n_blocks) {
         const long long per = std::max<long long>(1, std::min<long long>(n_blocks, (long long)(GCNT_BUDGET / smem)));
-        SF_RESERVE(ctx, G[G_GCNT], (size_t)per * smem);
+        TB2_RESERVE(ctx, "stats file", G[G_GCNT], (size_t)per * smem);
         a.gcnt = G[G_GCNT].as<int>();
         for (long long b0 = 0; b0 < n_blocks; b0 += per) {
             a.blk0 = (int)b0;
