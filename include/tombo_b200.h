@@ -733,6 +733,31 @@ int tb2_most_signif_get(tb2_ctx *ctx, double *key_out, double *frac_out, uint32_
                         uint32_t *cov_out, uint32_t *control_cov_out, uint32_t *valid_cov_out,
                         uint32_t *chrm_out, uint8_t *strand_out);
 
+/* ---- read filters (read_filter.cu; DESIGN.md §3 "Read filters") ----
+ * np.percentile(lens of read r, pctl[j]) into out[r * n_pctl + j], exactly numpy 2.3.5's
+ * default method='linear' (np.percentile in read_is_stuck, _filter_reads.py:61-69).  Read r
+ * holds lens[len_off[r] .. len_off[r + 1]) (the Events `length` column widened to int64).
+ * TB2_ERR_INVALID_ARG: n_pctl < 1, a percentile outside [0, 100], a negative len_off[0], or a
+ * read without lengths (len_off not strictly increasing). */
+int tb2_dwell_percentiles(tb2_ctx *ctx, int64_t n_reads, const int64_t *lens,
+                          const int64_t *len_off, int n_pctl, const double *pctl, double *out);
+/* The reversible filters of _io_and_map_read (resquiggle.py:1437-1453) on the resident batch
+ * after a successful tb2_batch_compute, over each read's final segs and sig_match_score.
+ * code[r]: -1 failed read, 1 sig_match_score > sig_match_thresh, 2 any
+ * np.percentile(np.diff(segs), pctl[j]) > thresh[j] (consulted only when not 1, the
+ * reference's elif), 0 kept.  n_pctl == 0: no observations-per-base filter.  pctl_out
+ * (nullable) gets the n_pctl percentiles of every successful read, NaN for failed ones.
+ * Before any compute, or after a failed one, TB2_ERR_INVALID_ARG. */
+int tb2_batch_read_filters(tb2_ctx *ctx, double sig_match_thresh, int n_pctl, const double *pctl,
+                           const double *thresh, int8_t *code, double *pctl_out);
+/* `tombo filter level_coverage` coverage (_filter_reads.py:112-126): reads of group g (one
+ * chromosome and strand) are grp_off[g] .. grp_off[g + 1], grp_off[0] = 0.  Each group's
+ * coverage has max(end) positions, every read of the group adds 1 over [start, end), and
+ * mid_cov[i] = cov[start + (end - start) / 2].  A read with start < 0 or end <= start is
+ * TB2_ERR_INVALID_ARG. */
+int tb2_read_mid_coverage(tb2_ctx *ctx, int64_t n_groups, const int64_t *grp_off,
+                          const int64_t *start, const int64_t *end, int64_t *mid_cov);
+
 #ifdef __cplusplus
 }
 #endif

@@ -182,6 +182,9 @@ _PROTOS = {
     'tb2_most_signif_add_aggregate': (_I, [_CTX]),
     'tb2_most_signif_count': (_I, [_CTX, pI64]),
     'tb2_most_signif_get': (_I, [_CTX, pF64, pF64, pU32, pU32, pU32, pU32, pU32, pU8]),
+    'tb2_dwell_percentiles': (_I, [_CTX, i64, pI64, pI64, _I, pF64, pF64]),
+    'tb2_batch_read_filters': (_I, [_CTX, f64, _I, pF64, pF64, pI8, pF64]),
+    'tb2_read_mid_coverage': (_I, [_CTX, i64, pI64, pI64, pI64, pI64]),
 }
 
 
@@ -1097,6 +1100,40 @@ class Context(object):
             ptr(c['strand'], C.c_uint8)))
         c['strand'] = c['strand'].view('S1')
         return c
+
+    # ---- read filters (read_filter.cu) -------------------------------------
+    def dwell_percentiles(self, lens, len_off, pctl):
+        """(n_reads, len(pctl)) array of np.percentile(lens[len_off[r]:len_off[r + 1]], p)"""
+        lens, len_off, pctl = as_i64(lens), as_i64(len_off), as_f64(np.atleast_1d(pctl))
+        n = len_off.shape[0] - 1
+        out = np.empty((max(n, 0), pctl.shape[0]))
+        self.check(self.lib.tb2_dwell_percentiles(self.handle, n, ptr(lens, i64), ptr(len_off, i64),
+                                                  pctl.shape[0], ptr(pctl, f64), ptr(out, f64)))
+        return out
+
+    def batch_read_filters(self, sig_match_thresh, obs_filter=None, want_percentiles=False):
+        """filter code of every read of the computed batch (-1 failed, 0 kept, 1 signal
+        matching, 2 observations per base) and, with want_percentiles, the (n_reads,
+        len(obs_filter)) percentiles of the successful reads"""
+        pairs = list(obs_filter or [])
+        pctl = as_f64([p for p, _ in pairs] or [0.0])
+        thresh = as_f64([t for _, t in pairs] or [0.0])
+        base_off = getattr(self, '_base_off', None)      # none before an upload: the call refuses
+        n = 0 if base_off is None else base_off.shape[0] - 1
+        code = np.empty(max(n, 1), dtype=np.int8)[:n]
+        pout = np.empty((n, len(pairs))) if want_percentiles else None
+        self.check(self.lib.tb2_batch_read_filters(
+            self.handle, float(sig_match_thresh), len(pairs), ptr(pctl, f64), ptr(thresh, f64),
+            ptr(code, C.c_int8), ptr(pout, f64) if pout is not None else None))
+        return (code, pout) if want_percentiles else code
+
+    def read_mid_coverage(self, grp_off, start, end):
+        """coverage at each read's middle, per (chromosome, strand) group of reads"""
+        grp_off, start, end = as_i64(grp_off), as_i64(start), as_i64(end)
+        out = np.empty(start.shape[0], dtype=np.int64)
+        self.check(self.lib.tb2_read_mid_coverage(self.handle, grp_off.shape[0] - 1, ptr(grp_off, i64),
+                                                  ptr(start, i64), ptr(end, i64), ptr(out, i64)))
+        return out
 
 
 def make_policy(kind='DNA', outlier_thresh=5.0, max_raw_cpts=200,

@@ -107,6 +107,8 @@ struct BatchResultView {
     const int *status;                  // status[r * stride]
     int stride;
     const long long *host_base_off;     // host copy of base_off (n_reads + 1)
+    const long long *segs;              // final segs, read r's nb + 1 at base_off[r] + r
+    const double *score;                // sig_match_score [n_reads]
 };
 int tb2_batch_result_view(tb2_ctx *ctx, BatchResultView *out);
 int tb2_region_accumulate_dev(tb2_ctx *ctx, long long n, const double *stats_dev,

@@ -60,6 +60,7 @@ struct KdeState;         // model_est.cu
 struct KmerModelState;   // kmer_model.cu
 struct AccuracyState;    // accuracy.cu
 struct StatsFileState;   // stats_file.cu
+struct ReadFilterState;  // read_filter.cu
 
 struct tb2_ctx {
     int device = 0;
@@ -83,6 +84,7 @@ struct tb2_ctx {
     std::shared_ptr<KmerModelState> kmer;
     std::shared_ptr<AccuracyState> accuracy;
     std::shared_ptr<StatsFileState> stats_file;
+    std::shared_ptr<ReadFilterState> read_filter;
     // tb2_resquiggle_batch pipelines large batches over two lanes (child contexts with
     // their own stream and buffers): H2D of chunk k+1 overlaps the kernels of chunk k
     std::vector<tb2_ctx *> lanes;

@@ -573,6 +573,8 @@ int tb2_batch_result_view(tb2_ctx *ctx, BatchResultView *out)
     out->status = &h->v.st[0].status;
     out->stride = (int)(sizeof(ReadState) / sizeof(int));
     out->host_base_off = h->hb.base_off.data();
+    out->segs = h->out_segs.as<long long>();
+    out->score = small_out(h->out_small, h->hb.n).score;
     return TB2_OK;
 }
 

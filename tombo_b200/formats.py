@@ -78,9 +78,11 @@ class ReadsIndex(object):
         return self.index_fn
 
 
-def load_index(index_fn, fast5s_dir, corr_grp='RawGenomeCorrected_000'):
+def load_index(index_fn, fast5s_dir, corr_grp='RawGenomeCorrected_000', remove_filtered=False):
     """{(chrm, strand): [readData]} from an index file (``_load_index_data``: 8-, 10- and
-    11-field records of the successive Tombo versions)"""
+    11-field records of the successive Tombo versions).  ``remove_filtered`` drops the reads
+    whose filtered flag is set, and then any (chrm, strand) left without reads, as
+    ``TomboReads(remove_filtered=True)`` does (tombo_helper.py:1296-1310)."""
     with io.open(index_fn, 'rb') as fp:
         raw = pickle.load(fp)
     if not raw:
@@ -97,6 +99,10 @@ def load_index(index_fn, fast5s_dir, corr_grp='RawGenomeCorrected_000'):
             rds.append(th.readData(start, end, filtered, rsrtr, strand,
                                    os.path.join(fast5s_dir, fn), corr_grp + '/' + s_grp, rna,
                                    *extra))
+        if remove_filtered:
+            rds = [rd for rd in rds if not rd.filtered]
+            if not rds:
+                continue
         out[(chrm, strand)] = rds
     return out
 

@@ -295,3 +295,25 @@ def resquiggle_reads(
     return _run_batch(list(map_results), std_ref, rsqgl_params, save_params, outlier_thresh,
                       max_raw_cpts, min_event_to_seq_ratio, const_scale, skip_seq_scaling,
                       seq_samp_type, max_scaling_iters, True, subsample_seed, device)
+
+
+def resquiggle_reads_for_index(
+        map_results, std_ref, rsqgl_params, save_params=None, index_sig_match_thresh=None,
+        obs_filter=None, seq_samp_type=th.seqSampleType(DNA_SAMP_TYPE, False), device=0,
+        **kwargs):
+    """:func:`resquiggle_reads`, then the reversible index filters of ``_io_and_map_read``
+    (resquiggle.py:1437-1453) on the same resident batch (``tb2_batch_read_filters``).
+
+    Returns ``(result, code)`` per read: ``result`` as :func:`resquiggle_reads` gives it,
+    ``code`` -1 for a failed read, 1 when ``sig_match_score > index_sig_match_thresh``
+    (``--signal-matching-score``; default ``SIG_MATCH_THRESH`` of the sample type), 2 when
+    a percentile of ``obs_filter`` ([[pctl, thresh]] or None) is above its threshold, 0
+    otherwise.  The start search keeps ``SIG_MATCH_THRESH`` whatever the index threshold."""
+    results = resquiggle_reads(map_results, std_ref, rsqgl_params, save_params,
+                               seq_samp_type=seq_samp_type, device=device, **kwargs)
+    if not results:
+        return []
+    thresh = (SIG_MATCH_THRESH[seq_samp_type.name] if index_sig_match_thresh is None
+              else index_sig_match_thresh)
+    codes = _lib.get_context(device).batch_read_filters(thresh, obs_filter)
+    return list(zip(results, (int(c) for c in codes)))

@@ -21,7 +21,8 @@ __all__ = [
     'channelInfo', 'dpResults', 'scaleValues', 'seqSampleType', 'regionStats', 'groupStats',
     'get_seq_kmers', 'rev_comp', 'warning_message', 'parse_locs_file', 'parse_motif_descs',
     'valid_cpts_w_cap', 'valid_cpts_w_cap_t_test', 'banded_traceback',
-    'adaptive_banded_forward_pass', 'get_raw_read_slot', 'get_multiple_slots_read_centric']
+    'adaptive_banded_forward_pass', 'get_raw_read_slot', 'get_multiple_slots_read_centric',
+    'status_message', 'get_mean_q_score', 'parse_obs_filter']
 
 SINGLE_LETTER_CODE = {
     'A': 'A', 'C': 'C', 'G': 'G', 'T': 'T', 'B': '[CGT]', 'D': '[AGT]', 'H': '[ACT]',
@@ -40,6 +41,35 @@ def warning_message(message):
     """tombo_helper.py:350-355"""
     sys.stderr.write('*' * 20 + ' WARNING ' + '*' * 20 + '\n\t' + message + '\n')
     sys.stderr.flush()
+
+
+def status_message(message, indent=False):
+    """tombo_helper.py:344-348"""
+    from time import strftime
+    sys.stderr.write(('\t' if indent else '') + strftime('[%H:%M:%S] ') + message + '\n')
+    sys.stderr.flush()
+
+
+PHRED_BASE = 33                                     # tombo_helper.py:53
+
+
+def get_mean_q_score(read_q):
+    """mean of a FASTQ quality string less the Phred offset (tombo_helper.py:389-394)"""
+    return np.mean([q_val - PHRED_BASE for q_val in read_q.encode('ASCII')])
+
+
+def parse_obs_filter(obs_filter):
+    """``--obs-per-base-filter`` ``pctl:thresh`` strings -> [[pctl, thresh]] or None
+    (tombo_helper.py:508-524); a percentile outside [0, 100] raises TomboError"""
+    if len(obs_filter) < 1:
+        return None
+    try:
+        obs_filter = [list(map(int, pctl_nobs.split(':'))) for pctl_nobs in obs_filter]
+    except Exception:
+        raise TomboError('Invalid format for observation filter')
+    if any(pctl < 0 or pctl > 100 for pctl, _ in obs_filter):
+        raise TomboError('Invalid percentile value.')
+    return obs_filter
 
 
 def _raise_status(st):

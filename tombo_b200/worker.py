@@ -25,6 +25,10 @@ from . import tombo_helper as th
 
 UNEXPECTED_ERROR = 'Unexpected error'       # resquiggle.py:1762
 MAX_NUM_UNEXP_ERRORS = 50                   # _MAX_NUM_UNEXP_ERRORS resquiggle.py:61
+POOR_MATCH_MESSAGE = ('Poor raw to expected signal matching '
+                      '(revert with `tombo filter clear_filters`)')      # resquiggle.py:1442
+OBS_FILTER_MESSAGE = ('Read filtered by observation per base '
+                      'thresholds (revert with `tombo filter clear_filters`)')   # :1451
 
 
 class ReadBatcher(object):
@@ -36,15 +40,29 @@ class ReadBatcher(object):
     order; ``message`` is what ``rsqgl_conn.send`` would have carried for that read."""
 
     def __init__(self, std_ref, rsqgl_params, save_params=None, max_reads=65536,
-                 max_samples=1 << 30, resquiggle_fn=None, **resquiggle_kwargs):
+                 max_samples=1 << 30, resquiggle_fn=None, index=None, corr_grp=None,
+                 bc_subgrp=None, index_sig_match_thresh=None, obs_filter=None,
+                 **resquiggle_kwargs):
         if max_reads < 1 or max_samples < 1:
             raise ValueError('max_reads and max_samples must be positive')
         self.std_ref, self.rsqgl_params, self.save_params = std_ref, rsqgl_params, save_params
         self.max_reads, self.max_samples = int(max_reads), int(max_samples)
         self.kwargs = resquiggle_kwargs
+        # index opt-in (_io_and_map_read, resquiggle.py:1425-1465): every successful read
+        # goes into ``index`` (a formats.ReadsIndex) with its filter flag, and the messages
+        # the reference queues on failed_reads_q collect in ``failed_reads``
+        self.index, self.corr_grp, self.bc_subgrp = index, corr_grp, bc_subgrp
+        self.failed_reads = []
+        if index is not None:
+            if corr_grp is None or bc_subgrp is None:
+                raise ValueError('the index needs corr_grp and bc_subgrp')
+            self.kwargs = dict(resquiggle_kwargs, index_sig_match_thresh=index_sig_match_thresh,
+                               obs_filter=obs_filter)
+        self.obs_filter = obs_filter
         if resquiggle_fn is None:
             from . import resquiggle as rsqgl        # needs the CUDA library: fail loudly
-            resquiggle_fn = rsqgl.resquiggle_reads
+            resquiggle_fn = rsqgl.resquiggle_reads_for_index if index is not None else \
+                rsqgl.resquiggle_reads
         self.resquiggle_fn = resquiggle_fn
         self._pending, self._samples = [], 0
         self.n_batches = 0
@@ -78,10 +96,12 @@ class ReadBatcher(object):
                                    % (len(results), len(pending)))
         except th.TomboError as e:
             # the batch call itself refused the input: every read reports that message
-            return [(fn, [True, [str(e), fn, True]]) for fn in fns]
+            return [self._failed(fn, str(e), True) for fn in fns]
         except Exception:
             tb = traceback.format_exc()
-            return [(fn, [True, [tb, fn, False]]) for fn in fns]
+            return [self._failed(fn, tb, False) for fn in fns]
+        if self.index is not None:
+            return [self._index_read(fn, res, code) for fn, (res, code) in zip(fns, results)]
         out = []
         for fn, res in zip(fns, results):
             if isinstance(res, th.TomboError):
@@ -91,6 +111,31 @@ class ReadBatcher(object):
             else:
                 out.append((fn, [False, res]))
         return out
+
+
+    def _failed(self, fn, message, is_tombo_error):
+        if self.index is not None:
+            self.failed_reads.append((message, self.bc_subgrp + ':::' + fn, is_tombo_error))
+        return (fn, [True, [message, fn, is_tombo_error]])
+
+    def _index_read(self, fn, res, code):
+        """one read of an index batch, as _io_and_map_read records it"""
+        if isinstance(res, Exception):
+            return self._failed(fn, str(res) if isinstance(res, th.TomboError) else repr(res),
+                                isinstance(res, th.TomboError))
+        key = self.bc_subgrp + ':::' + fn
+        if code == 1:
+            self.failed_reads.append((POOR_MATCH_MESSAGE, key, True))
+        elif self.obs_filter is not None:
+            # queued for every read tested, filtered or not (resquiggle.py:1446-1453)
+            self.failed_reads.append((OBS_FILTER_MESSAGE, key, True))
+        loc = res.genome_loc
+        rna = bool(self.kwargs.get('seq_samp_type', th.seqSampleType('DNA', False)).rev_sig)
+        self.index.add_read_data(loc.Chrom, loc.Strand, th.readData(
+            loc.Start, loc.Start + len(res.segs) - 1, code != 0, res.read_start_rel_to_raw,
+            loc.Strand, fn, self.corr_grp + '/' + self.bc_subgrp, rna, res.sig_match_score,
+            res.mean_q_score, res.align_info.ID))
+        return (fn, [False, res])
 
 
 def resquiggle_stream(reads, std_ref, rsqgl_params, save_params=None, **kwargs):
