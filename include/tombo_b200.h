@@ -758,6 +758,36 @@ int tb2_batch_read_filters(tb2_ctx *ctx, double sig_match_thresh, int n_pctl, co
 int tb2_read_mid_coverage(tb2_ctx *ctx, int64_t n_groups, const int64_t *grp_off,
                           const int64_t *start, const int64_t *end, int64_t *mid_cov);
 
+/* ---- genome browser tracks (browser_tracks.cu; DESIGN.md §3 "Genome browser tracks") ----
+ * Run-length coverage of `tombo text_output browser_files --file-types coverage`
+ * (TomboReads._compute_coverage + iter_coverage_regions, tombo_helper.py:1394-1453): reads of
+ * group g (one chromosome and strand) are grp_off[g] .. grp_off[g + 1], grp_off[0] = 0.  Each
+ * group's coverage has max(end) positions, every read adds 1 over [start, end), and is
+ * written as runs of equal coverage: run k of group g, for run_off[g] <= k < run_off[g + 1],
+ * starts at run_start[k] (0-based, within the group) with coverage run_cov[k], and lasts to
+ * the next run's start or to the group's max(end).  Zero-coverage runs are included.  A group
+ * of n_g reads has at most 2 n_g + 1 runs, so run_start and run_cov sized sum(2 n_g + 1)
+ * always suffice; run_off (n_groups + 1 entries) returns the real counts.  A read with
+ * start < 0 or end <= start is TB2_ERR_INVALID_ARG. */
+int tb2_coverage_runs(tb2_ctx *ctx, int64_t n_groups, const int64_t *grp_off, const int64_t *start,
+                      const int64_t *end, int64_t *run_off, int64_t *run_start, int64_t *run_cov);
+/* Per-position means of an Events slot over one chromosome and strand
+ * (get_mean_slot_genome_centric, tombo_helper.py:1661-1676), accumulated across calls.
+ * tb2_slot_sums_begin opens an accumulation of chrm_len positions (0 <= chrm_len <= 2^40),
+ * sums +0.0 and counts 0.  Each tb2_slot_sums_add then adds reads in order: read r holds
+ * vals[val_off[r] .. val_off[r + 1]), placed at start[r] onwards, reversed when reverse[r]
+ * (the - strand).  Every position's sum is the sequential fp64 sum of its values in read
+ * order across all calls, as the reference's slice-adds make it; NaN values are added and
+ * counted like any other.  start[r] < 0, start[r] + n_r > chrm_len or decreasing offsets are
+ * TB2_ERR_INVALID_ARG before anything runs, as is a position covered more than 2^31 - 1
+ * times; a failed add invalidates the accumulation.  tb2_slot_sums_means writes
+ * sums / (double)counts for all chrm_len positions (0 / 0 is NaN); without a begin, or after a
+ * failed add, it is TB2_ERR_INVALID_ARG. */
+int tb2_slot_sums_begin(tb2_ctx *ctx, int64_t chrm_len);
+int tb2_slot_sums_add(tb2_ctx *ctx, int64_t n_reads, const int64_t *start, const int64_t *val_off,
+                      const double *vals, const uint8_t *reverse);
+int tb2_slot_sums_means(tb2_ctx *ctx, double *out_mean);
+
 #ifdef __cplusplus
 }
 #endif

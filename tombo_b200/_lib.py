@@ -185,6 +185,10 @@ _PROTOS = {
     'tb2_dwell_percentiles': (_I, [_CTX, i64, pI64, pI64, _I, pF64, pF64]),
     'tb2_batch_read_filters': (_I, [_CTX, f64, _I, pF64, pF64, pI8, pF64]),
     'tb2_read_mid_coverage': (_I, [_CTX, i64, pI64, pI64, pI64, pI64]),
+    'tb2_coverage_runs': (_I, [_CTX, i64, pI64, pI64, pI64, pI64, pI64, pI64]),
+    'tb2_slot_sums_begin': (_I, [_CTX, i64]),
+    'tb2_slot_sums_add': (_I, [_CTX, i64, pI64, pI64, pF64, pU8]),
+    'tb2_slot_sums_means': (_I, [_CTX, pF64]),
 }
 
 
@@ -1133,6 +1137,39 @@ class Context(object):
         out = np.empty(start.shape[0], dtype=np.int64)
         self.check(self.lib.tb2_read_mid_coverage(self.handle, grp_off.shape[0] - 1, ptr(grp_off, i64),
                                                   ptr(start, i64), ptr(end, i64), ptr(out, i64)))
+        return out
+
+    # ---- genome browser tracks (browser_tracks.cu) -------------------------
+    def coverage_runs(self, grp_off, start, end):
+        """(run_off, run_start, run_cov): the coverage of each (chromosome, strand) group of
+        reads as runs of equal value; group g's runs are run_off[g] .. run_off[g + 1], each
+        starting at run_start (within the group) and lasting to the next start or max(end)"""
+        grp_off, start, end = as_i64(grp_off), as_i64(start), as_i64(end)
+        n_groups = grp_off.shape[0] - 1
+        bound = 2 * start.shape[0] + max(n_groups, 0)      # at most 2 n_g + 1 runs per group
+        run_off = np.zeros(max(n_groups, 0) + 1, dtype=np.int64)
+        run_start = np.empty(max(bound, 1), dtype=np.int64)
+        run_cov = np.empty(max(bound, 1), dtype=np.int64)
+        self.check(self.lib.tb2_coverage_runs(self.handle, n_groups, ptr(grp_off, i64), ptr(start, i64),
+                                              ptr(end, i64), ptr(run_off, i64), ptr(run_start, i64),
+                                              ptr(run_cov, i64)))
+        m = int(run_off[-1])
+        return run_off, run_start[:m], run_cov[:m]
+
+    def slot_means(self, chrm_len, batches):
+        """per-position means over chrm_len positions of the values of ``batches``, an
+        iterable of (start, val_off, vals, reverse) arrays added in order: read r of a batch
+        holds vals[val_off[r]:val_off[r + 1]] from start[r] on, reversed when reverse[r].
+        Each position's sum is the sequential fp64 sum of its values in read order; a
+        position no read covers is NaN."""
+        self.check(self.lib.tb2_slot_sums_begin(self.handle, int(chrm_len)))
+        for start, val_off, vals, reverse in batches:
+            start, val_off, vals = as_i64(start), as_i64(val_off), as_f64(vals)
+            reverse = np.ascontiguousarray(reverse, dtype=np.uint8)
+            self.check(self.lib.tb2_slot_sums_add(self.handle, start.shape[0], ptr(start, i64),
+                                                  ptr(val_off, i64), ptr(vals, f64), ptr(reverse, C.c_uint8)))
+        out = np.empty(max(int(chrm_len), 1))[:int(chrm_len)]
+        self.check(self.lib.tb2_slot_sums_means(self.handle, ptr(out, f64)))
         return out
 
 

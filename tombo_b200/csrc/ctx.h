@@ -61,6 +61,7 @@ struct KmerModelState;   // kmer_model.cu
 struct AccuracyState;    // accuracy.cu
 struct StatsFileState;   // stats_file.cu
 struct ReadFilterState;  // read_filter.cu
+struct BrowserTracksState;  // browser_tracks.cu
 
 struct tb2_ctx {
     int device = 0;
@@ -85,6 +86,7 @@ struct tb2_ctx {
     std::shared_ptr<AccuracyState> accuracy;
     std::shared_ptr<StatsFileState> stats_file;
     std::shared_ptr<ReadFilterState> read_filter;
+    std::shared_ptr<BrowserTracksState> browser_tracks;
     // tb2_resquiggle_batch pipelines large batches over two lanes (child contexts with
     // their own stream and buffers): H2D of chunk k+1 overlaps the kernels of chunk k
     std::vector<tb2_ctx *> lanes;

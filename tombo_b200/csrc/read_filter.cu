@@ -6,6 +6,8 @@
 //                           on the resident batch after tb2_batch_compute
 //   tb2_read_mid_coverage   the per-(chromosome, strand) coverage of `level_coverage` and each
 //                           read's mid-read value (_filter_reads.py:112-126)
+//   tb2_coverage_build      that coverage, the one builder of the project (coverage.h); also
+//                           behind tb2_coverage_runs (browser_tracks.cu)
 //
 // The percentiles take the two order statistics of numpy's linear interpolation from
 // tb2_block_select2 (select.cuh), one 256-thread block per read, reading the lengths from global
@@ -15,6 +17,7 @@
 #include "ctx.h"
 #include "batch.h"
 #include "read_filter.cuh"
+#include "coverage.h"
 #include <algorithm>
 #include <climits>
 #include <vector>
@@ -40,6 +43,61 @@ bool pctl_ok(int n_pctl, const double *pctl)
 unsigned grid_of(long long n, int nt) { return (unsigned)std::max<long long>(1, (n + nt - 1) / nt); }
 
 }  // namespace
+
+static_assert(B_END == B_START + COV_END && B_DIFF == B_START + COV_DIFF && B_TSUM == B_START + COV_TSUM &&
+              B_TOFF == B_START + COV_TOFF, "coverage workspace order");
+
+int tb2_coverage_build(tb2_ctx *ctx, const char *what, DevBuf *ws, int64_t n_groups, const int64_t *grp_off,
+                       const int64_t *start, const int64_t *end, std::vector<long long> &base)
+{
+    const int64_t n = grp_off[n_groups];
+    // absolute positions in the concatenated coverage arrays
+    std::vector<long long> as((size_t)n), ae((size_t)n);
+    base.assign((size_t)n_groups + 1, 0);
+    long long len = 0;
+    for (int64_t g = 0; g < n_groups; ++g) {
+        long long mx = 0;
+        for (int64_t i = grp_off[g]; i < grp_off[g + 1]; ++i) {
+            if (start[i] < 0 || end[i] <= start[i]) {
+                ctx->err = std::string(what) + ": every read needs 0 <= start < end";
+                return TB2_ERR_INVALID_ARG;
+            }
+            mx = std::max<long long>(mx, end[i]);
+        }
+        for (int64_t i = grp_off[g]; i < grp_off[g + 1]; ++i) { as[i] = len + start[i]; ae[i] = len + end[i]; }
+        len += grp_off[g + 1] > grp_off[g] ? mx + 1 : 0;
+        if (len > (1LL << 40)) { ctx->err = std::string(what) + ": coverage arrays too long"; return TB2_ERR_INVALID_ARG; }
+        base[(size_t)g + 1] = len;
+    }
+    const long long n_tiles = (len + RF_TILE - 1) / RF_TILE;
+    cudaStream_t q = ctx->stream;
+    TB2_RESERVE(ctx, what, ws[COV_DIFF], (size_t)len * 4);
+    TB2_RESERVE(ctx, what, ws[COV_TSUM], (size_t)n_tiles * 8);
+    TB2_RESERVE(ctx, what, ws[COV_TOFF], (size_t)(n_tiles + 1) * 8);
+    TB2_CUDA_TRY(ctx, ws[COV_START].upload(as.data(), (size_t)n, q));
+    TB2_CUDA_TRY(ctx, ws[COV_END].upload(ae.data(), (size_t)n, q));
+    int *cov = ws[COV_DIFF].as<int>();
+    TB2_CUDA_TRY(ctx, cudaEventRecord(ctx->ev0, q));
+    TB2_CUDA_TRY(ctx, cudaMemsetAsync(cov, 0, (size_t)len * 4, q));
+    k_rf_cov_diff<<<grid_of(n, 256), 256, 0, q>>>(ws[COV_START].as<long long>(), ws[COV_END].as<long long>(), n, cov);
+    TB2_CHECK_LAUNCH(ctx);
+    return tb2_coverage_scan(ctx, what, ws, cov, len);
+}
+
+int tb2_coverage_scan(tb2_ctx *ctx, const char *what, DevBuf *ws, int *x, long long len)
+{
+    const long long n_tiles = (len + RF_TILE - 1) / RF_TILE;
+    cudaStream_t q = ctx->stream;
+    TB2_RESERVE(ctx, what, ws[COV_TSUM], (size_t)n_tiles * 8);
+    TB2_RESERVE(ctx, what, ws[COV_TOFF], (size_t)(n_tiles + 1) * 8);
+    k_rf_tile_sum<<<(unsigned)n_tiles, RF_NT, 0, q>>>(x, len, ws[COV_TSUM].as<long long>());
+    TB2_CHECK_LAUNCH(ctx);
+    k_scan_offsets<long long><<<1, 1024, 0, q>>>(ws[COV_TSUM].as<long long>(), ws[COV_TOFF].as<long long>(), n_tiles);
+    TB2_CHECK_LAUNCH(ctx);
+    k_rf_tile_scan<<<(unsigned)n_tiles, RF_NT, 0, q>>>(x, len, ws[COV_TOFF].as<long long>());
+    TB2_CHECK_LAUNCH(ctx);
+    return TB2_OK;
+}
 
 extern "C" int tb2_dwell_percentiles(tb2_ctx *ctx, int64_t n_reads, const int64_t *lens,
                                      const int64_t *len_off, int n_pctl, const double *pctl,
@@ -126,45 +184,14 @@ extern "C" int tb2_read_mid_coverage(tb2_ctx *ctx, int64_t n_groups, const int64
     if (n > INT_MAX) { ctx->err = "read filters: more than 2^31 - 1 reads"; return TB2_ERR_INVALID_ARG; }
     if (n == 0) return TB2_OK;
     if (!start || !end || !mid_cov) return TB2_ERR_INVALID_ARG;
-    // absolute positions in the concatenated coverage arrays; group g's array has max(end) + 1
-    // entries (the last takes the -1 of the reads that end there)
-    std::vector<long long> as((size_t)n), ae((size_t)n);
-    long long base = 0;
-    for (int64_t g = 0; g < n_groups; ++g) {
-        long long mx = 0;
-        for (int64_t i = grp_off[g]; i < grp_off[g + 1]; ++i) {
-            if (start[i] < 0 || end[i] <= start[i]) {
-                ctx->err = "read filters: every read needs 0 <= start < end";
-                return TB2_ERR_INVALID_ARG;
-            }
-            mx = std::max<long long>(mx, end[i]);
-        }
-        for (int64_t i = grp_off[g]; i < grp_off[g + 1]; ++i) { as[i] = base + start[i]; ae[i] = base + end[i]; }
-        base += grp_off[g + 1] > grp_off[g] ? mx + 1 : 0;
-        if (base > (1LL << 40)) { ctx->err = "read filters: coverage arrays too long"; return TB2_ERR_INVALID_ARG; }
-    }
-    const long long len = base, n_tiles = (len + RF_TILE - 1) / RF_TILE;
     ReadFilterState &S = tb2_state(ctx->read_filter);
     DevBuf *B = S.buf;
     cudaStream_t q = ctx->stream;
-    TB2_RESERVE(ctx, "read filters", B[B_DIFF], (size_t)len * 4);
-    TB2_RESERVE(ctx, "read filters", B[B_TSUM], (size_t)n_tiles * 8);
-    TB2_RESERVE(ctx, "read filters", B[B_TOFF], (size_t)(n_tiles + 1) * 8);
     TB2_RESERVE(ctx, "read filters", B[B_MID], (size_t)n * 8);
-    TB2_CUDA_TRY(ctx, B[B_START].upload(as.data(), (size_t)n, q));
-    TB2_CUDA_TRY(ctx, B[B_END].upload(ae.data(), (size_t)n, q));
+    std::vector<long long> base;
+    if ((rc = tb2_coverage_build(ctx, "read filters", B + B_START, n_groups, grp_off, start, end, base))) return rc;
     int *cov = B[B_DIFF].as<int>();
     long long *ds = B[B_START].as<long long>(), *de = B[B_END].as<long long>();
-    TB2_CUDA_TRY(ctx, cudaEventRecord(ctx->ev0, q));
-    TB2_CUDA_TRY(ctx, cudaMemsetAsync(cov, 0, (size_t)len * 4, q));
-    k_rf_cov_diff<<<grid_of(n, 256), 256, 0, q>>>(ds, de, n, cov);
-    TB2_CHECK_LAUNCH(ctx);
-    k_rf_tile_sum<<<(unsigned)n_tiles, RF_NT, 0, q>>>(cov, len, B[B_TSUM].as<long long>());
-    TB2_CHECK_LAUNCH(ctx);
-    k_scan_offsets<long long><<<1, 1024, 0, q>>>(B[B_TSUM].as<long long>(), B[B_TOFF].as<long long>(), n_tiles);
-    TB2_CHECK_LAUNCH(ctx);
-    k_rf_tile_scan<<<(unsigned)n_tiles, RF_NT, 0, q>>>(cov, len, B[B_TOFF].as<long long>());
-    TB2_CHECK_LAUNCH(ctx);
     k_rf_mid<<<grid_of(n, 256), 256, 0, q>>>(ds, de, n, cov, B[B_MID].as<long long>());
     TB2_CHECK_LAUNCH(ctx);
     if ((rc = tb2_record_kernel_time(ctx))) return rc;

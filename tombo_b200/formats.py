@@ -107,6 +107,27 @@ def load_index(index_fn, fast5s_dir, corr_grp='RawGenomeCorrected_000', remove_f
     return out
 
 
+def load_reads_index(fast5s_dirs, corr_grp='RawGenomeCorrected_000', bc_subgrps=None):
+    """{(chrm, strand): [readData]} of ``TomboReads(fast5s_dirs, corr_grp, bc_subgrps)``
+    (tombo_helper.py:1292-1348) from the directories' Tombo indexes: filtered reads removed,
+    reads outside ``bc_subgrps`` (when given) dropped, a (chrm, strand) left without reads
+    dropped, and each (chrm, strand) concatenating its reads in directory order.  Groups come
+    in order of first appearance (the reference's follow a set).  A directory without an index
+    raises TomboError: building one from the FAST5 files is not done here."""
+    merged = OrderedDict()
+    for fast5s_dir in fast5s_dirs:
+        fast5s_dir = fast5s_dir if fast5s_dir.endswith('/') else fast5s_dir + '/'
+        index_fn = index_filename(fast5s_dir, corr_grp)
+        if not os.path.exists(index_fn):
+            raise th.TomboError('Tombo index file does not exist for ' + fast5s_dir)
+        for cs, rds in load_index(index_fn, fast5s_dir, corr_grp, remove_filtered=True).items():
+            if bc_subgrps is not None:
+                rds = [rd for rd in rds if rd.corr_group.split('/')[-1] in bc_subgrps]
+            if rds:
+                merged.setdefault(cs, []).extend(rds)
+    return dict(merged)
+
+
 # ---------------------------------------------------------------------------
 # per-read statistics blocks
 # ---------------------------------------------------------------------------

@@ -22,7 +22,9 @@ __all__ = [
     'get_seq_kmers', 'rev_comp', 'warning_message', 'parse_locs_file', 'parse_motif_descs',
     'valid_cpts_w_cap', 'valid_cpts_w_cap_t_test', 'banded_traceback',
     'adaptive_banded_forward_pass', 'get_raw_read_slot', 'get_multiple_slots_read_centric',
-    'status_message', 'get_mean_q_score', 'parse_obs_filter']
+    'status_message', 'get_mean_q_score', 'parse_obs_filter', 'get_chrm_sizes',
+    'get_single_slot_read_centric', 'get_single_slot_genome_centric', 'get_mean_slot_genome_centric',
+    'iter_mean_slot_values', 'iter_coverage_regions']
 
 SINGLE_LETTER_CODE = {
     'A': 'A', 'C': 'C', 'G': 'G', 'T': 'T', 'B': '[CGT]', 'D': '[AGT]', 'H': '[ACT]',
@@ -363,6 +365,113 @@ def get_multiple_slots_read_centric(r_data, slot_names, corr_grp=None):
         return [events[name] for name in slot_names]
     except Exception:
         return [None] * len(slot_names)
+
+
+# ---- genome browser tracks (tombo text_output browser_files) ----
+SLOT_BATCH_VALUES = 1 << 24          # Events values per tb2_slot_sums_add call
+
+
+def get_chrm_sizes(reads_index, ctrl_reads_index=None):
+    """covered length of every chromosome: the largest read end over both strands and both
+    samples (tombo_helper.py:396-421); ``reads_index`` is {(chrm, strand): [readData]}"""
+    strand_chrm_sizes = {}
+    for ri in (reads_index, ctrl_reads_index):
+        if ri is None:
+            continue
+        for (chrm, strand), cs_reads in ri.items():
+            if len(cs_reads) == 0:
+                continue
+            strand_chrm_sizes.setdefault(chrm, []).append(max(rd.end for rd in cs_reads))
+    return dict((chrm, max(sizes)) for chrm, sizes in strand_chrm_sizes.items())
+
+
+def get_single_slot_read_centric(r_data, slot_name, corr_grp=None):
+    """one read-centric Events column, or None when it cannot be read (tombo_helper.py:1678-1700)"""
+    return get_multiple_slots_read_centric(r_data, [slot_name], corr_grp)[0]
+
+
+def get_single_slot_genome_centric(r_data, slot_name):
+    """the column in genome order: reversed on the - strand (tombo_helper.py:1702-1712)"""
+    r_slot_values = get_single_slot_read_centric(r_data, slot_name)
+    if r_slot_values is None:
+        return None
+    if r_data.strand == '-':
+        r_slot_values = r_slot_values[::-1]
+    return r_slot_values
+
+
+def _slot_batches(cs_reads, slot_name, max_values):
+    """(start, val_off, vals, reverse) batches of at most ``max_values`` values (one read may
+    exceed it alone), reading one read's Events at a time; unreadable reads are skipped"""
+    starts, lens, vals, rev, n = [], [], [], [], 0
+    for r_data in cs_reads:
+        r_vals = get_single_slot_read_centric(r_data, slot_name)
+        if r_vals is None:
+            continue
+        r_vals = np.asarray(r_vals, dtype=np.float64)
+        if n and n + r_vals.shape[0] > max_values:
+            yield (np.array(starts, np.int64), np.concatenate([[0], np.cumsum(lens)]).astype(np.int64),
+                   np.concatenate(vals), np.array(rev, np.uint8))
+            starts, lens, vals, rev, n = [], [], [], [], 0
+        starts.append(r_data.start)
+        lens.append(r_vals.shape[0])
+        vals.append(r_vals)
+        rev.append(r_data.strand == '-')
+        n += r_vals.shape[0]
+    if starts:
+        yield (np.array(starts, np.int64), np.concatenate([[0], np.cumsum(lens)]).astype(np.int64),
+               np.concatenate(vals), np.array(rev, np.uint8))
+
+
+def get_mean_slot_genome_centric(cs_reads, chrm_len, slot_name, ctx=None, device=0,
+                                 max_values=SLOT_BATCH_VALUES):
+    """mean of ``slot_name`` over the reads at every position of one chromosome and strand
+    (tombo_helper.py:1714-1729): tb2_slot_sums_*, fed one read at a time in batches of at most
+    ``max_values`` values.  Each position is the sequential fp64 sum of its values in read
+    order divided by their count; NaN values count, and uncovered positions are NaN.  A read
+    whose values run past ``chrm_len`` raises, as numpy's slice-add does."""
+    ctx = ctx if ctx is not None else _lib.get_context(device)
+    return ctx.slot_means(chrm_len, _slot_batches(cs_reads, slot_name, max_values))
+
+
+def iter_mean_slot_values(reads_index, chrm_sizes, slot_name, ctrl_reads_index=None, ctx=None,
+                          device=0):
+    """(chrm, strand, means, control means) over sorted(chrm) x ('+', '-')
+    (tombo_helper.py:1731-1765): without a control, only the covered groups; with one, the
+    groups either sample covers, None for the sample that does not"""
+    for chrm, strand in [(c, s) for c in sorted(chrm_sizes) for s in ('+', '-')]:
+        cs = (chrm, strand)
+        if ctrl_reads_index is None:
+            if cs not in reads_index:
+                continue
+            yield chrm, strand, get_mean_slot_genome_centric(
+                reads_index[cs], chrm_sizes[chrm], slot_name, ctx, device), None
+        else:
+            means = ctrl_means = None
+            if cs in reads_index:
+                means = get_mean_slot_genome_centric(reads_index[cs], chrm_sizes[chrm], slot_name, ctx, device)
+            if cs in ctrl_reads_index:
+                ctrl_means = get_mean_slot_genome_centric(
+                    ctrl_reads_index[cs], chrm_sizes[chrm], slot_name, ctx, device)
+            if means is None and ctrl_means is None:
+                continue
+            yield chrm, strand, means, ctrl_means
+
+
+def iter_coverage_regions(reads_index, ctx=None, device=0):
+    """(chrm, strand, cs_cov, cs_cov_starts) of every group in index order
+    (TomboReads.iter_coverage_regions, tombo_helper.py:1430-1453): the coverage levels of the
+    runs and their starts, closed by max(end).  One tb2_coverage_runs call for all groups."""
+    ctx = ctx if ctx is not None else _lib.get_context(device)
+    keys = [cs for cs, cs_reads in reads_index.items() if len(cs_reads) > 0]
+    grp_off = np.concatenate([[0], np.cumsum([len(reads_index[cs]) for cs in keys])]).astype(np.int64)
+    start = np.array([rd.start for cs in keys for rd in reads_index[cs]], dtype=np.int64)
+    end = np.array([rd.end for cs in keys for rd in reads_index[cs]], dtype=np.int64)
+    run_off, run_start, run_cov = ctx.coverage_runs(grp_off, start, end)
+    for g, (chrm, strand) in enumerate(keys):
+        a, b = run_off[g], run_off[g + 1]
+        cs_end = end[grp_off[g]:grp_off[g + 1]].max()
+        yield chrm, strand, run_cov[a:b], np.concatenate([run_start[a:b], [cs_end]])
 
 
 # ---- FAST5 Events table: the output seam of the resquiggle path (SURVEY 8(f)-3) ----
