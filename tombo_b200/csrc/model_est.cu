@@ -38,43 +38,6 @@ struct KdeState { DevBuf buf[K_COUNT]; };
 
 namespace {
 
-// summand i of a pairwise sum computed on the fly by g(o + i): indexable and offsettable
-// like an array, so tb2_pairwise_sum (common.cuh) takes it
-template <class G> struct Terms {
-    G g;
-    int o;
-    __device__ __forceinline__ double operator[](int i) const { return g(o + i); }
-    __device__ __forceinline__ Terms operator+(int k) const { return Terms{g, o + k}; }
-};
-
-// numpy's pairwise sum of f(0) .. f(n - 1) by one warp: the top five levels of numpy's
-// split tree give each lane one subtree, summed by tb2_pairwise_sum in numpy's order; the
-// subtree sums are then added back up the same tree (left + right).  A node of 128 or fewer
-// summands is not split: the lane on its left edge owns it.  Every lane returns the total.
-template <class F> __device__ double warp_pairwise_sum(const F &f, int n)
-{
-    const int lane = threadIdx.x & 31;
-    int o = 0, len = n;
-    bool own = true;
-    unsigned split = 0;                        // bit d: this lane's depth-d node was split
-    for (int d = 0; d < 5; ++d) {
-        const bool right = (lane >> (4 - d)) & 1;
-        if (len > 128) {
-            split |= 1u << d;
-            const int n2 = tb2_pairwise_split(len);
-            if (right) { o += n2; len -= n2; } else len = n2;
-        } else if (right) {
-            own = false;
-        }
-    }
-    double v = own ? tb2_pairwise_sum(Terms<F>{f, o}, len) : 0.0;
-    for (int d = 4; d >= 0; --d) {
-        const double r = __shfl_down_sync(TB2_FULL_MASK, v, 1 << (4 - d));
-        if ((split >> d) & 1) v = v + r;        // meaningful on the left child's lane
-    }
-    return __shfl_sync(TB2_FULL_MASK, v, 0);
-}
-
 // one warp per set
 __global__ void __launch_bounds__(128)
 k_kde_setup(const double *lv, const long long *off, long long n_sets, double bw, double norm0,

@@ -21,12 +21,15 @@ __device__ __forceinline__ double tb2_unkey(unsigned long long k)
     return __longlong_as_double((long long)u);
 }
 
+struct Sum4 { unsigned int x, y, z, w; };
+
 struct SelectSmem {
     unsigned int hist[256];
     unsigned int warp_tot[8];
     unsigned int sel_bin, sel_below, sel_cnt;
     unsigned long long red_u64[8], red_and[8];
     unsigned int red_u32[8];
+    Sum4 red_sum4[8];
     unsigned long long small[TB2_SEL_SMALL];   // finishing list of the radix select
     unsigned long long result, result2;   // rank k; rank k + 1 when it sat in the same list
     unsigned int n_small, have2;
@@ -44,6 +47,29 @@ __device__ __forceinline__ unsigned int tb2_block_sum(unsigned int v, SelectSmem
     unsigned int t = 0;
 #pragma unroll
     for (int w = 0; w < TB2_SEL_THREADS / 32; ++w) t += sm.red_u32[w];
+    return t;
+}
+
+// four block-wide sums at once, for the barriers of one
+__device__ __forceinline__ Sum4 tb2_block_sum4(Sum4 v, SelectSmem &sm)
+{
+    const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+#pragma unroll
+    for (int off = 16; off > 0; off >>= 1) {
+        v.x += __shfl_xor_sync(TB2_FULL_MASK, v.x, off);
+        v.y += __shfl_xor_sync(TB2_FULL_MASK, v.y, off);
+        v.z += __shfl_xor_sync(TB2_FULL_MASK, v.z, off);
+        v.w += __shfl_xor_sync(TB2_FULL_MASK, v.w, off);
+    }
+    __syncthreads();
+    if (lane == 0) sm.red_sum4[warp] = v;
+    __syncthreads();
+    Sum4 t = {0u, 0u, 0u, 0u};
+#pragma unroll
+    for (int w = 0; w < TB2_SEL_THREADS / 32; ++w) {
+        const Sum4 q = sm.red_sum4[w];
+        t.x += q.x; t.y += q.y; t.z += q.z; t.w += q.w;
+    }
     return t;
 }
 

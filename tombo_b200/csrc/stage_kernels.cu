@@ -62,7 +62,8 @@ int tb2_launch_normalize(tb2_ctx *ctx, const BatchView &b, const StagePolicy &po
 int tb2_launch_cpts(tb2_ctx *ctx, const BatchView &b, const tb2_params &p, int on_raw)
 {
     // bit sets of the greedy pass: 4 + (min_obs_per_base - 1) words per 32 candidates, in
-    // shared memory when the longest read of the batch fits in 48 KB (else the read's scratch)
+    // shared memory when the longest read of the batch fits in 48 KB (else the read's scratch);
+    // the rest of CP_SMEM_BYTES holds the candidate scores of the reads whose scores fit too
     if (!p.use_t_test_seg) {
         k_cumsum<<<(b.n_reads + CS_WARPS - 1) / CS_WARPS, CS_WARPS * 32, 0, ctx->stream>>>(b, on_raw);
         TB2_CHECK_LAUNCH(ctx);
@@ -70,6 +71,7 @@ int tb2_launch_cpts(tb2_ctx *ctx, const BatchView &b, const tb2_params &p, int o
     const long long nw = (b.max_raw + 32) / 32;
     long long words = (4 + std::max(0, (int)p.min_obs_per_base - 1)) * nw;
     if (words * 4 > 48 * 1024) words = 0;   // the default dynamic shared-memory limit
+    words = std::max(words, (long long)(CP_SMEM_BYTES - sizeof(SelectSmem) - sizeof(int)) / 4);
     k_cpts<<<b.n_reads, ST_THREADS, (size_t)words * 4, ctx->stream>>>(b, p, on_raw, (int)words);
     TB2_CHECK_LAUNCH(ctx);
     return TB2_OK;

@@ -166,38 +166,45 @@ k_normalize(BatchView b, StagePolicy pol, int first_call)
         if (threadIdx.x == 0) s.status = TB2_ERR_UNEXPECTED;
         return;
     }
-    for (int i = threadIdx.x; i < n; i += ST_THREADS) norm[i] = (raw[i] - shift) / scale;  // :554
-    __syncthreads();
     // the resquiggle path never passes a threshold with scale values (segment_signal);
     // normalize_raw_signal(outlier_thresh=t, scale_values=sv) does (thresh_with_sv)
     const double thresh = (given && !pol.thresh_with_sv) ? NAN : pol.outlier_thresh;
-    if (!isnan(thresh)) {                                                             // :559-563
-        double med, mad;
-        if ((n & 1) && !use_const && !given) {
-            // odd n: shift is an element of raw and scale an element of |raw - shift|.
-            // x -> (x - shift) / scale is monotone (each rounding is), so the middle
-            // order statistic of norm is the image of shift: (shift - shift) / scale = +0;
-            // |norm - 0| = |x - shift| / scale is monotone in |x - shift|, so its middle
-            // order statistic is scale / scale = 1 -- the values np.median returns.
-            med = 0.0;
-            mad = 1.0;
-        } else {
-            // even n with raw's own shift: the two middle elements of norm are the images
-            // of raw's; supplied shift / scale need not be raw's medians, so select on norm
-            if ((n & 1) || given) med = tb2_block_median([&](int i) { return norm[i]; }, n, sm);
-            else med = (((mid_a - shift) / scale) + ((mid_b - shift) / scale)) / 2.0;
-            mad = tb2_block_median([&](int i) { return fabs(norm[i] - med); }, n, sm);
-        }
+    // odd n with raw's own shift and scale: shift is an element of raw and scale an element
+    // of |raw - shift|.  x -> (x - shift) / scale is monotone (each rounding is), so the
+    // middle order statistic of norm is the image of shift: (shift - shift) / scale = +0;
+    // |norm - 0| = |x - shift| / scale is monotone in |x - shift|, so its middle order
+    // statistic is scale / scale = 1 -- the values np.median returns.
+    const bool closed = !isnan(thresh) && (n & 1) && !use_const && !given;
+    if (closed) {                                                                     // :559-563
+        const double med = 0.0, mad = 1.0;
         lo = med - (mad * thresh);
         hi = med + (mad * thresh);
-    } else if (given) { lo = s.sv.lower_lim; hi = s.sv.upper_lim; }                   // :565-566
-    if (!isnan(lo) && !isnan(hi)) {
-        for (int i = threadIdx.x; i < n; i += ST_THREADS) {
-            const double v = norm[i];
-            norm[i] = v > hi ? hi : (v < lo ? lo : v);
-        }
+    } else if (isnan(thresh) && given) { lo = s.sv.lower_lim; hi = s.sv.upper_lim; }  // :565-566
+    // limits known before norm exists: normalise and clip in one pass over the signal
+    const bool limits_first = closed || isnan(thresh);
+    const bool clip_first = limits_first && !isnan(lo) && !isnan(hi);
+    for (int i = threadIdx.x; i < n; i += ST_THREADS) {
+        const double v = (raw[i] - shift) / scale;                                    // :554
+        norm[i] = clip_first ? (v > hi ? hi : (v < lo ? lo : v)) : v;
     }
     __syncthreads();
+    if (!limits_first) {                                                              // :559-563
+        // even n with raw's own shift: the two middle elements of norm are the images
+        // of raw's; supplied shift / scale need not be raw's medians, so select on norm
+        double med;
+        if ((n & 1) || given) med = tb2_block_median([&](int i) { return norm[i]; }, n, sm);
+        else med = (((mid_a - shift) / scale) + ((mid_b - shift) / scale)) / 2.0;
+        const double mad = tb2_block_median([&](int i) { return fabs(norm[i] - med); }, n, sm);
+        lo = med - (mad * thresh);
+        hi = med + (mad * thresh);
+        if (!isnan(lo) && !isnan(hi)) {
+            for (int i = threadIdx.x; i < n; i += ST_THREADS) {
+                const double v = norm[i];
+                norm[i] = v > hi ? hi : (v < lo ? lo : v);
+            }
+        }
+        __syncthreads();
+    }
     if (threadIdx.x == 0) {
         s.sv.shift = shift; s.sv.scale = scale; s.sv.lower_lim = lo; s.sv.upper_lim = hi;
         s.sv.outlier_thresh = thresh;
@@ -283,6 +290,9 @@ __device__ __forceinline__ uint32_t cp_shl(const uint32_t *x, int w, int o)
 }
 
 #define CP_MAX_OFF 12   // exclusion zones up to +-12 candidates run bit-parallel
+// shared memory of one k_cpts block, static and dynamic: five blocks (the launch bounds) fit
+// an SM's 228 KB with their 1 KB reserve each
+#define CP_SMEM_BYTES (44 * 1024)
 
 __global__ void __launch_bounds__(ST_THREADS, 5)
 k_cpts(BatchView b, tb2_params p, int on_raw, int smem_words)
@@ -298,21 +308,24 @@ k_cpts(BatchView b, tb2_params p, int on_raw, int smem_words)
     const int n = (int)(b.raw_off[r + 1] - ro);
     const double *sig = (on_raw ? b.rawf : b.norm) + ro;
     double *cs = b.cs + ro + r;
-    double *sc = b.scores + ro;
     const int w = (int)p.running_stat_width, m = (int)p.min_obs_per_base;
     const int N = s.num_events;
-    int n_cand, bound;
+    // num_cands = candidate_poss.shape[0] - 2*w (:105-106); :199
+    const int n_cand = p.use_t_test_seg ? n - 2 * w : n + 1 - 2 * w;
+    const int bound = p.use_t_test_seg ? n_cand : n_cand - 2 * w;
+    if (n_cand <= 0) { if (tid == 0) s.status = TB2_ERR_UNEXPECTED; return; }
+    const int nw = (n_cand + 31) >> 5;
+    const int no = m - 1;                       // zone half-width
+    const int bit_words = (4 + max(no, 0)) * nw;
+    // the candidate scores stay on chip when they fit beside this read's bit sets (scores
+    // first: 8-byte aligned), else they go to the read's slice of b.scores
+    const bool sc_on_chip = 2 * n_cand + bit_words <= smem_words;
+    double *sc = sc_on_chip ? reinterpret_cast<double *>(cp_smem) : b.scores + ro;
     if (!p.use_t_test_seg) {
-        n_cand = n + 1 - 2 * w;
-        bound = n_cand - 2 * w;  // num_cands = candidate_poss.shape[0] - 2*w (:105-106)
-        if (n_cand <= 0) { if (tid == 0) s.status = TB2_ERR_UNEXPECTED; return; }
         // cs = np.cumsum(concatenate([[0.0], signal])) comes from k_cumsum
         for (int i = tid; i < n_cand; i += ST_THREADS)
             sc[i] = fabs(((2 * cs[i + w]) - cs[i]) - cs[i + 2 * w]);   // :95-98
     } else {
-        n_cand = n - 2 * w;
-        bound = n_cand;      // :199
-        if (n_cand <= 0) { if (tid == 0) s.status = TB2_ERR_UNEXPECTED; return; }
         for (int pos = tid; pos < n_cand; pos += ST_THREADS) {           // :153-179
             double m1 = 0, m2 = 0, var1 = 0, var2 = 0, d;
             for (int k = 0; k < w; ++k) m1 += sig[pos + k];
@@ -336,10 +349,9 @@ k_cpts(BatchView b, tb2_params p, int on_raw, int smem_words)
     // undecided higher-ranked candidate, and rejects those with an accepted one in
     // their zone (Jacobi sweep on double buffers: decisions are final and are exactly
     // the ranked greedy's, whatever the sweep order).
-    const int nw = (n_cand + 31) >> 5;
-    const int no = m - 1;                       // zone half-width
     uint32_t *bits;
-    if ((4 + max(no, 0)) * nw <= smem_words) bits = cp_smem;
+    if (sc_on_chip) bits = cp_smem + 2 * n_cand;
+    else if (bit_words <= smem_words) bits = cp_smem;
     else bits = reinterpret_cast<uint32_t *>(b.cstate + ((2 * ro + 128LL * r + 3) & ~3LL));
     if (no > CP_MAX_OFF) { if (tid == 0) s.status = TB2_ERR_CAPACITY; return; }
     uint32_t *A0 = bits, *A1 = bits + nw, *D0 = bits + 2 * nw, *D1 = bits + 3 * nw, *G = bits + 4 * nw;
@@ -414,10 +426,8 @@ k_cpts(BatchView b, tb2_params p, int on_raw, int smem_words)
         }
         g += acc && v > vN;
     }
-    g = tb2_block_sum(g, sm);
-    e = tb2_block_sum(e, sm);
-    eq_all = tb2_block_sum(eq_all, sm);
-    higher = tb2_block_sum(higher, sm);
+    const Sum4 tot = tb2_block_sum4(Sum4{g, e, eq_all, higher}, sm);
+    g = tot.x; e = tot.y; eq_all = tot.z; higher = tot.w;
     const int need = N - (int)g;   // 1 <= need <= e, taken from the largest positions
     int posN;
     if (e == 1u) {
@@ -1624,10 +1634,15 @@ k_theil_sen(BatchView b, StagePolicy pol, int first_call)
 // final re-normalisation + per-base means + sig_match_score
 // (resquiggle.py:1190-1199, get_read_seg_score tombo_stats.py:2327-2338)
 // ===========================================================================
-__global__ void __launch_bounds__(ST_THREADS)
+#define FIN_STAGE 2048   // per-base |z| held in shared memory (16 KB) up to this many bases
+
+// eight blocks per SM (32 registers): the per-base loop waits on its loads, and more resident
+// reads hide that better than the registers the bound costs (a few spill slots)
+__global__ void __launch_bounds__(ST_THREADS, 8)
 k_finalize(BatchView b, StagePolicy pol, int first_call, double *norm_mean_out,
            double *norm_signal_out)
 {
+    __shared__ double s_t[FIN_STAGE];
     const int r = blockIdx.x;
     ReadState &s = b.st[r];
     if (!rd_active(s)) return;
@@ -1637,7 +1652,7 @@ k_finalize(BatchView b, StagePolicy pol, int first_call, double *norm_mean_out,
     const int *segs = b.segs + bo + r;
     const bool rescale = !(first_call && pol.skip_seq_scaling);
     const double shc = s.shc, scc = s.scc;
-    double *t = b.tmp_b + bo + r;
+    double *t = nb <= FIN_STAGE ? s_t : b.tmp_b + bo + r;
     for (int i = threadIdx.x; i < nb; i += ST_THREADS) {
         const int a = segs[i], z = segs[i + 1];
         double acc = 0;
@@ -1655,6 +1670,10 @@ k_finalize(BatchView b, StagePolicy pol, int first_call, double *norm_mean_out,
             o[k] = rescale ? (norm[k] - shc) / scc : norm[k];
     }
     __syncthreads();
-    if (threadIdx.x == 0) s.score = tb2_pairwise_sum(t, nb) / (double)nb;
+    // np.mean's pairwise sum, one lane per subtree of numpy's split tree
+    if (threadIdx.x < 32) {
+        const double sum = warp_pairwise_sum([t](int i) { return t[i]; }, nb);
+        if (threadIdx.x == 0) s.score = sum / (double)nb;
+    }
 }
 
